@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- diffusion-steps/sec of the CLIP-guided sampling step (BASELINE.json metric) on N B200s.
+"""bench.py -- diffusion-steps/sec of the CLIP-guided sampling step (BASELINE.json metric) on N H100s.
 
     python bench.py --gpus 1 --steps 20 --warmup 5                       # this framework, cfg2 per GPU
+    python bench.py --gpus 1 --steps 20 --warmup 5 --dump-outputs DIR    # ... and write the last timed step's outputs as DIR/*.npy
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference --steps K --warmup W               # the oracle port on the host CPU cores
 
@@ -50,7 +51,7 @@ DOMINANT = dict(M=65536, N=256, K=2304)  # 256^2 x 256ch conv3x3: 31 % of the UN
 
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    fb = dict(burst=1590.0, sustained=1400.0, hbm=6650.0, src="fallback")  # B200_PROFILING.md's stated fallback
+    fb = dict(burst=989.0, sustained=989.0, hbm=3350.0, src="fallback: H100 SXM data sheet (dense FP16, 700 W)")
     if os.path.exists(p):
         try:
             d = json.load(open(p))
@@ -62,7 +63,7 @@ def peaks():
 
 
 class ClockSampler:
-    """SM clock / throttle reasons during the timed region (B200_PROFILING.md).  NVML from a sampling thread (one query ~50 us, every
+    """SM clock / throttle reasons during the timed region.  NVML from a sampling thread (one query ~50 us, every
     10 ms: a 250 ms timed region yields ~25 samples); `nvidia-smi -lms 200` as the fallback when pynvml is not usable."""
 
     NAMES = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
@@ -161,7 +162,7 @@ def build_engine(device, rank, world):
 
 def dominant_kernel_time(device, reps=24):
     """Average duration of the dominant conv launch (256x256 pixels, 256 -> 256 channels, 3x3), rotating over buffers that
-    together exceed the 126 MB L2, CUDA events on the launching stream."""
+    together exceed the 50 MB L2, CUDA events on the launching stream."""
     from clip_guided_diffusion_b200.plan import Plan, pack_conv
     th.manual_seed(0)
     plan = Plan()
@@ -214,6 +215,25 @@ def conv_share(eng, mode, reps=3):
     return e0.elapsed_time(e1) * 1e-3 / reps, flop, len(ks)
 
 
+DUMP_LIMIT = 64 << 20  # bytes of .npy data written by --dump-outputs
+
+
+def dump_outputs(out_dir, out, gathered):
+    """What the timed path returned in its last timed step, as float32 DIR/<name>.npy: every tensor of the step's result dict
+    (`sample`, `pred_xstart`, ...) and the gathered final images.  The inputs of a run are fixed by its arguments (seeded weights,
+    targets and per-step draws), so two builds can be compared output for output."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: v for k, v in out.items() if isinstance(v, th.Tensor)}
+    arrays["gathered_images"] = gathered
+    total = 0
+    for name, t in sorted(arrays.items()):
+        a = t.detach().float().cpu().numpy()
+        total += a.nbytes
+        if total > DUMP_LIMIT:
+            raise RuntimeError(f"--dump-outputs: {name} would take the dump past {DUMP_LIMIT >> 20} MB")
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 def run_ours(args):
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
@@ -231,6 +251,8 @@ def run_ours(args):
     T = diff.num_timesteps
     y0 = th.zeros(eng.global_batch, dtype=th.long)
 
+    last = {}
+
     def step_resident(i, img):
         # x_t is fresh synthetic noise every step: with random (non-denoising) weights a chained trajectory diverges within a
         # few steps (pred_xstart ~ 1e3 and growing), which says nothing about throughput; timing is value-independent
@@ -238,6 +260,7 @@ def run_ours(args):
         y = eng.draw_classes()
         out = eng.fused_step(diff, MODE, i, img, y, cond, 0.0)
         cond.current_timestep = max(cond.current_timestep - 1, 0)
+        last["out"] = out
         return out["sample"]
 
     # ---------------- device-resident loop (value)
@@ -270,6 +293,8 @@ def run_ours(args):
     clocks = sampler.stop() if rank == 0 else None
     ms_total = float(ms.item())
     finite = bool(th.isfinite(img).all()) and tuple(gathered.shape) == (eng.global_batch, 3, eng.H, eng.W)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["out"], gathered)
 
     # ---------------- end-to-end loop: host buffers, H2D of x_t and D2H of the sample inside every step
     host_x = th.empty(B, 3, eng.H, eng.W, pin_memory=True)
@@ -332,14 +357,14 @@ def run_ours(args):
         "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_total / args.steps, "higher_is_better": True,
         "scaling": "weak", "vs_baseline": None, "dtype": "fp16 (fp32 accumulate / norm / softmax / sampler)", "data": "synthetic (x_t ~ N(0,1) redrawn every step, seeded random weights)",
         "config": {"workload": CFG["name"] + ", class-cond UNet, seeded random weights", "global_batch": eng.global_batch, "parallelism": f"dp{world} (batch shard, no data-path collective)",
-                   "l2": "per-step working set (2.3 GB of packed weights + activations) exceeds the 126 MB L2; no explicit flush",
+                   "l2": "per-step working set (2.3 GB of packed weights + activations) exceeds the 50 MB L2; no explicit flush",
                    "finite": finite},
         "e2e": {"value": e2e, "unit": "image-steps/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h, "ms_per_step": ms_e2e / args.steps},
         "gpu_launches": launches * args.steps,
         "launches_per_step": launches,
         "clocks": clocks,
         "roofline": {"bound": "tensor", "achieved": ach, "peak": pk["burst"], "unit": "TFLOP/s", "frac": ach / pk["burst"], "traffic": traffic,
-                     "kernel": "conv_tc2_kernel<256> 256x256x256->256 3x3 (M=65536,N=256,K=2304)", "peak_source": pk["src"] + " burst (kernel timed alone)",
+                     "kernel": "conv_tc_kernel<256> 256x256x256->256 3x3 (M=65536,N=256,K=2304)", "peak_source": pk["src"] + " burst (kernel timed alone)",
                      "avg_launch_s": t_dom},
         "step_tensor_frac": CFG["tflop"] * 1e12 * value / world / (pk["sustained"] * 1e12),
     }
@@ -366,7 +391,7 @@ _CPU_THREADS = None
 
 def pick_cpu_threads() -> int:
     """Deterministic thread count of the CPU arms: every host core up to 32 (PyTorch's CPU convs stop scaling there: the build box'
-    8 cores take 30 s/step, the B200 host ran 5-6 s/step with 16-48 threads and 206 s/step with 128; CGD_CPU_THREADS overrides)."""
+    8 cores take 30 s/step; CGD_CPU_THREADS overrides)."""
     global _CPU_THREADS
     if _CPU_THREADS is None:
         _CPU_THREADS = int(os.environ.get("CGD_CPU_THREADS", "0")) or min(os.cpu_count() or 1, 32)
@@ -489,8 +514,7 @@ def cpu_baseline(sample_steps=3):
 def run_reference(args):
     """The reference's own algorithm on the host cores (fp32 oracle port: guided_diffusion / clip / lpips are not installable
     offline, DESIGN.md section 5).  Same metric / unit / config strings as our arm; --warmup W untimed steps, --steps K timed ones.
-    One cfg2 step is 5-6 s on the B200 host: W + K steps fit a few minutes; on a slower host the run is cut to a time budget and
-    says so (`steps` / `warmup` then report what actually ran)."""
+    On a slow host the run is cut to a time budget and says so (`steps` / `warmup` then report what actually ran)."""
     if int(os.environ.get("RANK", "0")) != 0:
         return
     unet, diff, cond = oracle_cpu_setup()
@@ -537,6 +561,8 @@ def main():
     ap.add_argument("--no-torch-baseline", action="store_true", help="skip the PyTorch-CUDA (cuDNN/cuBLAS eager autograd) oracle-port arm")
     ap.add_argument("--torch-baseline", action="store_true", help="(default now; kept for old command lines)")
     ap.add_argument("--workload", default="cfg2", choices=sorted(WORKLOADS), help="per-GPU shard of a BASELINE.json configuration (default: the metric's)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     global CFG
     CFG = WORKLOADS[args.workload]

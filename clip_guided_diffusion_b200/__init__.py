@@ -1,4 +1,4 @@
-"""clip_guided_diffusion_b200 -- B200 (sm_100a) implementation of the CLIP-guided diffusion sampling step.
+"""clip_guided_diffusion_b200 -- H100 (sm_90a) implementation of the CLIP-guided diffusion sampling step.
 
 Host side is Python (PyTorch tensors for device memory, streams and torch.distributed); every per-timestep kernel
 lives in libcgd_b200.so (include/cgd_b200.h) and is loaded with ctypes.  No CPU / PyTorch fallback exists for the

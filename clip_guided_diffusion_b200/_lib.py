@@ -46,7 +46,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise CgdError(f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                       "(nvcc, sm_100a).  There is no CPU / PyTorch fallback for the sampling step.")
+                       "(nvcc, sm_90a).  There is no CPU / PyTorch fallback for the sampling step.")
     lib = ctypes.CDLL(LIB_PATH)
     lib.cgd_last_error.restype = ctypes.c_char_p
     lib.cgd_abi_version.restype = ctypes.c_int
@@ -64,7 +64,7 @@ def load():
         getattr(lib, name).argtypes = [vp, vp]
     for name in ("cgd_unet_destroy", "cgd_vit_destroy", "cgd_step_destroy"):
         getattr(lib, name).argtypes = [vp]
-    if lib.cgd_abi_version() != 1:
+    if lib.cgd_abi_version() != 2:
         raise CgdError("libcgd_b200.so ABI version mismatch")
     _lib = lib
     return lib

@@ -1,4 +1,4 @@
-"""Build libcgd_b200.so in-tree with nvcc for sm_100a (no torch extension machinery: the library is a plain
+"""Build libcgd_b200.so in-tree with nvcc for sm_90a (H100; no torch extension machinery: the library is a plain
 C-ABI shared object loaded with ctypes)."""
 from __future__ import annotations
 
@@ -10,8 +10,8 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libcgd_b200.so")
-SOURCES = ["api.cu", "conv_tc.cu", "conv_tc2.cu", "conv_tc3.cu", "conv_narrow.cu", "norm.cu", "norm_fused.cu", "norm_grid.cu", "norm_grid2.cu", "norm_stream.cu", "elementwise.cu", "attention.cu", "attention_small.cu", "attention_mma.cu", "attention_wide.cu", "guidance.cu", "augs.cu", "lpips.cu", "linear_small.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+SOURCES = ["api.cu", "conv_tc.cu", "conv_narrow.cu", "norm.cu", "norm_fused.cu", "norm_grid.cu", "norm_grid2.cu", "norm_stream.cu", "elementwise.cu", "attention.cu", "attention_small.cu", "attention_mma.cu", "attention_wide.cu", "guidance.cu", "augs.cu", "lpips.cu", "linear_small.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "--use_fast_math=false"]
 
 
@@ -56,7 +56,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         list(ex.map(cc, jobs))
     objs = [os.path.join(objdir, src.replace(".cu", ".o")) for src in SOURCES]
     if force or jobs or _stale(LIB, objs):
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs + ["-Xcompiler", "-fPIC", "-cudart", "static"]
+        cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB] + objs + ["-Xcompiler", "-fPIC", "-cudart", "static"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,4 +1,4 @@
-"""``clip_guided_diffusion(...)`` -- the reference's orchestrator surface (cgd/cgd.py:19-283) over the B200 engine.
+"""``clip_guided_diffusion(...)`` -- the reference's orchestrator surface (cgd/cgd.py:19-283) over the H100 engine.
 
 Same keyword arguments and the same generator contract (yields ``(batch_idx, png_path)``); set-up stays Python and
 runs once (seed, prompt encoding, weight loading, cutout cache), the per-timestep work is the engine's fused step.
@@ -137,7 +137,7 @@ def _tower_config(clip_sd: dict):
 
 def _require_cuda(device):
     if not str(device).startswith("cuda") or not th.cuda.is_available():
-        raise RuntimeError("clip_guided_diffusion_b200 runs the sampling step on a CUDA (sm_100a) device only; there is no CPU path")
+        raise RuntimeError("clip_guided_diffusion_b200 runs the sampling step on a CUDA (sm_90a, H100) device only; there is no CPU path")
 
 
 def clip_guided_diffusion(

@@ -173,7 +173,7 @@ extern "C" {
 
 int cgd_abi_version(void) { return CGD_ABI_VERSION; }
 const char* cgd_last_error(void) { return cgd::g_err; }
-int cgd_conv_cluster_capacity(int32_t bn, int32_t splits) { return cgd::conv_tc3_max_clusters(bn, splits); }
+int cgd_conv_cluster_capacity(int32_t bn, int32_t splits) { return cgd::conv_cluster_capacity(bn, splits); }
 
 int cgd_plan_create(const CgdOp* ops, int32_t n_ops, void** plan_out) {
   Plan* pl = nullptr;

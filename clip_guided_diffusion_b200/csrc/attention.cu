@@ -400,7 +400,7 @@ int launch_attn_bwd(const CgdOp& op, cudaStream_t st) {
 
 // ================================================================================================
 // Tensor-core attention for long sequences (T % 256 == 0: the 32x32 and 16x16 UNet levels).
-// S = Q K^T, O = P V and the four backward products run as batched GEMMs on the tcgen05 CTA-pair kernel (conv_tc2.cu,
+// S = Q K^T, O = P V and the four backward products run as batched GEMMs on the wgmma conv kernel (conv_tc.cu,
 // CGD_OP_CONV with a batched B operand); the kernels below are the glue: batched fp16 transposes (so that every GEMM
 // operand is K-major), the fp32 row softmax (fp16 in/out like the reference's `softmax(w.float()).type(w.dtype)`), and
 // its backward dS = P * (dP - rowsum(P * dP)) * scale.

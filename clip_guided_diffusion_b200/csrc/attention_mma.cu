@@ -3,9 +3,8 @@
 //
 // Replaces [3P] guided-diffusion QKVAttention(Legacy) at the 32x32 / 16x16 UNet levels (T = 1024 / 256) and [3P] CLIP
 // nn.MultiheadAttention's core for ViT-B/16, L/14 (T = 197, 257) (SURVEY.md K4, K14).  Nothing T x T touches HBM.
-// History (profiles/r01_launches_cfg2_step_v7_warm.csv): the same math as batched tcgen05 GEMMs (S and P materialised, K = 64 per
-// GEMM, explicit transposes, row softmax kernels) cost ~1.3 ms per step in ~110 launches of 7 - 66 TFLOP/s; the fp32 CUDA-core
-// flash kernels before that 4.6 ms.  Structure of the backward (as in attention.cu): delta = rowsum(dO * O); one kernel per key
+// The alternative, batched tensor-core GEMMs (plan.tc_attention: S and P materialised, K = 64 per GEMM, explicit transposes, row
+// softmax kernels), needs ~110 launches per step and a T x T round trip through memory.  Structure of the backward (as in attention.cu): delta = rowsum(dO * O); one kernel per key
 // tile accumulates dK, dV over the query tiles, one CTA per query tile accumulates dQ over the key tiles (same launch).
 #include <cuda_fp16.h>
 

@@ -3,8 +3,8 @@
 //
 // Replaces [3P] CLIP nn.MultiheadAttention's core for ViT-B/32 (50 tokens) and [3P] guided-diffusion QKVAttention(Legacy) at the
 // 8x8 UNet level (64 tokens) (SURVEY.md K4, K14).  Why a separate kernel: these problems are one 64x64 tile per head -- the
-// tcgen05 pair kernel wants 256-row tiles (conv_tc2.cu) and the fp32 CUDA-core flash kernels of attention.cu spend 17 us
-// (forward) and 62 us (backward, three launches) on 192 such tiles (profiles/r01_launches_cfg2_step_v5_warm.csv).  Here the
+// wgmma conv kernel wants 128-row tiles (conv_tc.cu) and the fp32 CUDA-core flash kernels of attention.cu need three launches
+// for the backward of such tiles.  Here the
 // whole backward -- S, P, dP, dS, dQ, dK, dV -- is one launch; P and dS go through shared memory once (fp16, like the
 // reference's fp16 attention weights) to feed the transposed products.
 #include <cuda_fp16.h>

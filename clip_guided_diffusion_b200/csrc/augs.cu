@@ -242,7 +242,7 @@ __global__ void cutouts_aug_bwd_kernel(const __half* __restrict__ dpatch, const 
 
 static inline int aug_blocks(int64_t items) {
   int64_t b = ceil_div(items, 256);
-  return (int)std::max<int64_t>(1, std::min<int64_t>(b, 148 * 16));
+  return (int)std::max<int64_t>(1, std::min<int64_t>(b, 132 * 16));
 }
 
 // op tables: include/cgd_b200.h CGD_OP_CUTOUTS_AUG_FWD / _BWD

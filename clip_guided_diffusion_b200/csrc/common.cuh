@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for libcgd_b200 (sm_100a only).
+// common.cuh -- shared device helpers for libcgd_b200 (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -7,15 +7,15 @@
 
 #include "../../include/cgd_b200.h"
 
-#ifndef __CUDA_ARCH_FEAT_SM100_ALL
+#ifndef __CUDA_ARCH_FEAT_SM90_ALL
 #if defined(__CUDA_ARCH__)
-#error "libcgd_b200 must be compiled for sm_100a (-gencode arch=compute_100a,code=sm_100a)"
+#error "libcgd_b200 must be compiled for sm_90a (-gencode arch=compute_90a,code=sm_90a)"
 #endif
 #endif
 
 namespace cgd {
 
-typedef __half act_t;  // activation / weight storage type of the networks (UMMA kind::f16, fp32 accumulate)
+typedef __half act_t;  // activation / weight storage type of the networks (wgmma fp16 operands, fp32 accumulate)
 
 // ---------------------------------------------------------------- error plumbing (host)
 void set_error(const char* fmt, ...);
@@ -62,12 +62,12 @@ struct DeviceOnce {
   }
   int get() const { return value[cur()]; }
 };
-// SM count of the current device (148 on a full B200; grids of the persistent kernels are sized from it, not from the constant)
+// SM count of the current device (132 on an H100 SXM; grids of the persistent kernels are sized from it, not from the constant)
 static inline int device_sm_count() {
   static DeviceOnce once;
   if (once.needed()) {
     int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
     once.mark(sms);
   }
   return once.get();
@@ -114,10 +114,9 @@ __device__ __forceinline__ float rcp_ftz(float x) {
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// sigmoid(v) = 1/2 + 1/2 tanh(v / 2): ONE MUFU op (tanh.approx.f32, relative error 2^-11) instead of two (ex2 + rcp).  Why it matters
-// (ncu, profiles/r02_families_summary.txt): the XU (SFU) pipe was 56 % busy in the streaming GroupNorm-apply kernel -- two MUFU per
-// element at 16 lanes / clk / SM put a ~20 us floor under a kernel whose 67 MB of traffic need ~12 us; every SiLU / SiLU' in the
-// GroupNorm kernels is XU-bound the same way.  Accuracy: |sigmoid error| <= 2.5e-4 absolute, i.e. |silu error| <= 2.5e-4 |v| -- the
+// sigmoid(v) = 1/2 + 1/2 tanh(v / 2): ONE MUFU op (tanh.approx.f32, relative error 2^-11) instead of two (ex2 + rcp).  Why it matters:
+// the SFU issues 16 lanes / clk / SM, so two MUFU ops per element can put a floor under a streaming GroupNorm-apply kernel that is
+// higher than its memory traffic; every SiLU / SiLU' in the GroupNorm kernels has the same per-element cost.  Accuracy: |sigmoid error| <= 2.5e-4 absolute, i.e. |silu error| <= 2.5e-4 |v| -- the
 // size of the fp16 rounding of the output itself; the full-size parity tests (tests/test_gpu_baseline_configs.py) bound the effect.
 // -DCGD_SIGMOID_EX2RCP restores the two-MUFU form (A/B builds).
 __device__ __forceinline__ float tanh_approx(float x) {
@@ -137,29 +136,10 @@ __device__ __forceinline__ float silu_grad_f(float v) {
   return s * (1.f + v * (1.f - s));
 }
 
-// packed fp32 pairs (FFMA2 / FMUL2 / FADD2 in SASS, sm_100+): two lanes per issue slot for the issue-bound normalisation kernels
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-  float2 d;
-  asm("{.reg .b64 ra, rb, rc, rd; mov.b64 ra, {%2, %3}; mov.b64 rb, {%4, %5}; mov.b64 rc, {%6, %7}; fma.rn.f32x2 rd, ra, rb, rc; "
-      "mov.b64 {%0, %1}, rd;}"
-      : "=f"(d.x), "=f"(d.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-  return d;
-}
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-  float2 d;
-  asm("{.reg .b64 ra, rb, rd; mov.b64 ra, {%2, %3}; mov.b64 rb, {%4, %5}; mul.rn.f32x2 rd, ra, rb; mov.b64 {%0, %1}, rd;}"
-      : "=f"(d.x), "=f"(d.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return d;
-}
-__device__ __forceinline__ float2 add2(float2 a, float2 b) {
-  float2 d;
-  asm("{.reg .b64 ra, rb, rd; mov.b64 ra, {%2, %3}; mov.b64 rb, {%4, %5}; add.rn.f32x2 rd, ra, rb; mov.b64 {%0, %1}, rd;}"
-      : "=f"(d.x), "=f"(d.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return d;
-}
+// fp32 pairs, one rounding per lane
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 #ifdef CGD_SIGMOID_EX2RCP
 // silu on a pair: t * 1 / (1 + 2^(-log2e * t))
 __device__ __forceinline__ float2 silu2(float2 t) {
@@ -195,8 +175,8 @@ __device__ __forceinline__ float2 silu_grad2(float2 t) {
 // ---------------------------------------------------------------- global-memory barrier among co-resident CTAs
 // bar[0] = arrival count (returns to 0), bar[1] = generation (only ever incremented): reusable across launches / graph replays
 // without a reset.  Called by ONE thread per CTA after a block-level barrier; acquire / release atomics instead of
-// __threadfence(): the three MEMBAR.SC.GPU of a fence-based version cost ~5 us per barrier on B200 (each invalidates the L1),
-// which made a 148-CTA barrier ~7 us (profiles/r01_gn_microbench_v2.txt: 14.5 us for a 1 MB GroupNorm).
+// __threadfence(): each MEMBAR.SC.GPU of a fence-based version invalidates the L1, which makes a barrier over every SM of the
+// device cost several microseconds.
 __device__ __forceinline__ void global_barrier_arrive_wait(unsigned int* bar, unsigned int n) {
   unsigned int gen, old, cur;
   asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(gen) : "l"(bar + 1) : "memory");  // before arriving: cannot advance yet

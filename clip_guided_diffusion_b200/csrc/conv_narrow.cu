@@ -1,9 +1,8 @@
 // conv_narrow.cu -- 3x3 convolution with at most 8 output channels and an fp32 (NCHW) output: the UNet head (256 -> 6, [3P] `out[2]`)
 // and the stem's input gradient (256 -> 3, the last op of the backward that cgd/cgd.py:228 triggers).
 //
-// Why a separate kernel (profiles/r02_launches_v1_warm.csv): on the implicit-GEMM pair kernel these two layers take 55 us each -- the
-// N = 16 tile uses 1/16 of the tensor width while the A operand (33.5 MB) is still streamed nine times, once per tap, from L2
-// (302 MB per launch).  Here a CTA owns a 4 x 32 pixel tile: per 64-channel slice its (4+2) x (32+2) halo is loaded ONCE into shared
+// Why a separate kernel: on the wgmma tile kernel the N = 16 tile of these two layers uses 1/16 of the tensor width while the A operand
+// (33.5 MB at 256x256) is still streamed nine times, once per tap, from L2 (302 MB per launch).  Here a CTA owns a 4 x 32 pixel tile: per 64-channel slice its (4+2) x (32+2) halo is loaded ONCE into shared
 // memory (cp.async, zero-filled outside the image = the conv padding), the nine taps are shifted ldmatrix reads of that tile, and the
 // product runs on mma.sync.m16n8k16 whose N = 8 is exactly this layer's width.  A traffic: 1.6x the tensor (halo), 53 MB instead of
 // 302 MB.  fp16 operands, fp32 accumulate, like the other conv paths.
@@ -112,7 +111,7 @@ conv_narrow_kernel(const __half* __restrict__ A, const __half* __restrict__ Wp, 
 bool conv_narrow_eligible(const ConvTcLaunch& L) {
   const ConvTcParams& p = L.p;
   return p.taps == 9 && p.Cout <= 8 && p.Cin % 64 == 0 && p.Cin <= 1024 && p.out_f32 && p.res == nullptr && p.splits == 1 && !p.b_batched &&
-         (L.impl == 0 || L.impl == 3) && L.ldb % 8 == 0;
+         L.impl == 0 && L.ldb % 8 == 0;
 }
 
 int conv_narrow_launch(const ConvTcLaunch& L, cudaStream_t st) {
@@ -133,11 +132,10 @@ int conv_narrow_launch(const ConvTcLaunch& L, cudaStream_t st) {
 // ================================================================================================ 8 x 8 images: weight-streaming kernel
 // conv_small_kernel -- 3x3 / 1x1 convolution of an 8 x 8 image (M = 64 pixels): the UNet's deepest level and its attention 1x1s.
 //
-// Why (profiles/r02_launches_v3_warm.csv): on the tcgen05 tiles these layers are 64 pixels in a 128- / 256-row tile, split 8 - 16 ways
-// along K with an fp32 workspace and a reduce launch (or a 16-CTA cluster): 18.6 us for the 1024 -> 1024 3x3 (18.9 MB of weights =
-// 4 us at HBM speed), 10 - 18 us for the 1x1s -- 56 launches, ~1 ms per step of pure latency.  Here the problem is turned around: a CTA
+// Why: on the wgmma tiles these layers are 64 pixels in a 128-row tile, split many ways along K with an fp32 workspace and a reduce
+// launch (or a cluster), so their time is launch and reduction latency rather than the weight stream (18.9 MB for the 1024 -> 1024 3x3).  Here the problem is turned around: a CTA
 // owns EIGHT OUTPUT CHANNELS of one image and the whole K extent -- no split-K, no reduction, one launch.  Its 8 x K weight slab
-// (<= 148 KB) is fetched with cp.async BEFORE the grid dependency resolves (weights are step-invariant: under programmatic dependent
+// (at most 8 x 9216 halfs) is fetched with cp.async BEFORE the grid dependency resolves (weights are step-invariant: under programmatic dependent
 // launch the HBM stream overlaps the previous kernel's tail), the activations stream through a 4-stage ring of 64-channel slices (halo
 // tile for 3x3), and the product runs on mma.sync.m16n8k16 whose N = 8 is exactly the CTA's channel slab: 8 warps = 4 pixel tiles x 2
 // halves of every slice's K, two independent accumulator chains per warp, one shared-memory add at the end.
@@ -145,9 +143,8 @@ constexpr int SM_THREADS = 256, SM_STAGES = 4;
 
 // Data movement: per 64-channel slice ONE TMA tensor load of the box [64 ch x 10 x 10 x 1] anchored at (-1, -1) -- the 8 x 8 image with
 // its zero border, out-of-image coordinates zero-filled by the TMA unit, 128-byte swizzle (slot = pixel, 16-byte chunk ^= slot & 7) --
-// and eight cp.async.bulk copies for the weight slab (one row of K halfs per output channel).  Measured on the way here
-// (profiles/r02_call_s_small_v*.log): every 16-byte piece as its own cp.async (~22 k requests per CTA): 20 us, request-bound; one 128-byte
-// cp.async.bulk per pixel (1024 per CTA): 43 us -- small bulk copies cost ~40 ns each in the TMA unit.
+// and eight cp.async.bulk copies for the weight slab (one row of K halfs per output channel): a few large requests rather than one
+// cp.async per 16-byte piece or one small bulk copy per pixel, which would make the kernel request-bound.
 template <int TAPS>
 __global__ void __launch_bounds__(SM_THREADS)
 conv_small_kernel(const __grid_constant__ CUtensorMap tmA, const __half* __restrict__ Wp, const float* __restrict__ bias,
@@ -256,7 +253,7 @@ static inline int conv_small_smem(int taps, int Cin) {  // 1024-byte aligned sta
 bool conv_small_eligible(const ConvTcLaunch& L) {
   const ConvTcParams& p = L.p;
   return (p.taps == 9 || p.taps == 1) && p.H == 8 && p.W == 8 && p.Cin % 64 == 0 && p.Cout % 8 == 0 && !p.out_f32 && p.out_sc == 1 && !p.b_batched &&
-         p.res_mode == 0 && p.epi_stats == nullptr && (L.impl == 0 || L.impl == 3) && L.ldb % 8 == 0 && p.out_sw % 2 == 0 &&
+         p.res_mode == 0 && p.epi_stats == nullptr && L.impl == 0 && L.ldb % 8 == 0 && p.out_sw % 2 == 0 &&
          (p.res == nullptr || p.res_sw % 2 == 0) && L.a_sn % 8 == 0 && L.a_sh % 8 == 0 && L.a_sw % 8 == 0 &&
          (reinterpret_cast<uintptr_t>(L.A) % 16) == 0 && (reinterpret_cast<uintptr_t>(L.Wp) % 16) == 0 && conv_small_smem(p.taps, p.Cin) <= 212 * 1024;
 }

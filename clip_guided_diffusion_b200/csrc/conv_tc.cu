@@ -1,4 +1,4 @@
-// conv_tc.cu -- implicit-GEMM convolution / GEMM on Blackwell tcgen05 tensor cores.
+// conv_tc.cu -- implicit-GEMM convolution / GEMM on Hopper wgmma tensor cores.
 //
 // Replaces (forward and input-gradient directions) the [3P] guided-diffusion UNet Conv2d 3x3 / 1x1 and
 // Conv1d k=1 layers and the [3P] CLIP ViT Linear / patch-conv layers that the reference runs through
@@ -8,31 +8,34 @@
 // 128-pixel x BN-channel output tile; the 128 pixels are a TW x TH x TN box of the image grid.
 // For every filter tap and every 64-channel slice of the input, one TMA 4-D tiled load fetches the
 // (dx,dy)-shifted box -- out-of-image coordinates are zero-filled by the TMA unit, which *is* the
-// conv padding -- into a 128B-swizzled K-major shared-memory tile; one 2-D TMA load fetches the
-// matching [BN x 64] slice of the pre-packed weights.  A single thread issues
-// tcgen05.mma.cta_group::1.kind::f16 (M=128, N=BN, K=16) x4 per stage, accumulating in TMEM.
-// Pipeline: STAGES-deep smem ring with full/empty mbarriers (TMA producer warp <-> MMA warp),
-// tcgen05.commit releases stages and finally signals the 4 epilogue warps, which read the
-// accumulator with tcgen05.ld (32 lanes x 32 columns), add bias / residual and store fp16.
-// Small-M layers (8x8, 16x16 feature maps with K up to 18k) use split-K over gridDim.z with an fp32
-// workspace and a reduce kernel, so that the weight stream is spread over many SMs.
+// conv padding -- into a 128B-swizzled K-major shared-memory tile; one TMA load fetches the matching
+// [BN x 64] slice of the pre-packed weights.  Warp 8 is the TMA producer; warps 0-7 are two consumer
+// warpgroups, each issuing wgmma.m64nBNk16 x4 per stage for its 64 pixel rows and accumulating in
+// registers.  Pipeline: STAGES-deep smem ring with full/empty mbarriers; a stage is released once
+// the wgmma group that read it has retired (wait_group 1 keeps one group in flight).
+// Epilogue: the accumulators go to an fp32 staging tile that reuses the ring; then each consumer thread
+// owns one pixel row and half of the tile's channels and adds bias / residual, stores fp16 / fp32.
+// Small-M layers (8x8 .. 32x32 feature maps, long-K Linears) split K over gridDim.z: either into an
+// fp32 workspace summed by a reduce kernel, or (CONV i23 = 1) inside a thread-block cluster of
+// `splits` CTAs that sum each other's staging tiles through distributed shared memory -- one launch,
+// no workspace; CTA s of the cluster finishes columns [s*BN/S, (s+1)*BN/S) of the tile.
 #include <cuda.h>
 #include <stdlib.h>
 
 #include <algorithm>
 
 #include "common.cuh"
-#include "conv_splitk.cuh"
-#include "conv_sched.cuh"
 #include "conv_tc.cuh"
 #include "pdl.cuh"
 #include "tc_ptx.cuh"
+#include "wgmma_ptx.cuh"
 
 namespace cgd {
 
 // ---------------------------------------------------------------- kernel
 constexpr int BM = 128, BK = 64;
-constexpr int kThreads = 192;  // warp0 TMA, warp1 MMA (+TMEM alloc), warps 2..5 epilogue
+constexpr int kConsumers = 256;            // warps 0..7: two wgmma warpgroups of 64 pixel rows each
+constexpr int kThreads = kConsumers + 32;  // warp 8: TMA producer
 
 template <int BN>
 struct TcCfg {
@@ -40,8 +43,12 @@ struct TcCfg {
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kTmemCols = BN <= 32 ? 32 : (BN <= 64 ? 64 : (BN <= 128 ? 128 : 256));
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int kStageLd = BN + 4;  // fp32 staging row stride (floats): 16-byte aligned rows, rows shifted across banks
+  static constexpr int kStagingBytes = BM * kStageLd * 4;
+  static constexpr int kAuxBytes = 256 /*barriers*/ + BN * 4 /*epilogue statistics exchange: 4 row quarters x BN/8 octets x 2*/;
+  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + kAuxBytes;
+  static_assert(kStagingBytes <= kStages * kStageBytes, "the fp32 staging tile reuses the operand ring");
+  static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 };
 
 template <int BN>
@@ -52,10 +59,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + Cfg::kStages * Cfg::kABytes;
+  float* staging = reinterpret_cast<float*>(smem);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
   uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* tmem_full_bar = empty_bar + Cfg::kStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
+  float* stat_red = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes + 256);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -67,39 +74,29 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int w0 = tw_i * p.TW, h0 = th_i * p.TH, n0 = tn_i * p.TN;
   const int ncol0 = blockIdx.y * BN;
   const int kb0 = blockIdx.z * p.kb_per_split;
-  const int kb1 = min(kb0 + p.kb_per_split, p.kblocks);
+  const int kb1 = min(kb0 + p.kb_per_split, p.kblocks);  // non-empty for every split (host)
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], kConsumers / 32);  // one arrive per consumer warp
     }
-    mbar_init(tmem_full_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"((uint32_t)Cfg::kTmemCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
   pdl_launch_dependents();
 
-  if (warp == 0) {
+  if (warp == kConsumers / 32) {
     // ===== TMA producer
     if (lane == 0) {
       const int cblks = p.Cin / BK;
       int stage = 0;
       uint32_t phase = 0;
       for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
+        mbar_wait_trap(&empty_bar[stage], phase ^ 1);
         mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
         const int tap = kb / cblks, cb = kb - tap * cblks;
         int dy = 0, dx = 0;
@@ -108,116 +105,164 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           dx = tap % 3 - 1;
         }
         tma_load_4d(smem_a + stage * Cfg::kABytes, &tmA, &full_bar[stage], cb * BK, w0 + dx, h0 + dy, n0);
-        tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmB, &full_bar[stage], kb * BK, ncol0);
+        tma_load_4d(smem_b + stage * Cfg::kBBytes, &tmB, &full_bar[stage], kb * BK, ncol0, p.b_batched ? h0 : 0, p.b_batched ? n0 : 0);
         if (++stage == Cfg::kStages) {
           stage = 0;
           phase ^= 1;
         }
       }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer (single thread)
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint64_t da = make_smem_desc_sw128(smem_u32(smem_a + stage * Cfg::kABytes));
-        const uint64_t db = make_smem_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes));
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          // advance 16 elements (32 B) along K inside the 128 B swizzle row: +2 in the (>>4) address field
-          tc_mma_f16(tmem_base, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-        }
-        tc_commit(&empty_bar[stage]);  // frees this smem stage once the MMAs above have read it
-        if (++stage == Cfg::kStages) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      tc_commit(tmem_full_bar);  // accumulator complete
+    } else if (p.pf_bytes > 0) {
+      l2_prefetch_slice(p.pf_ptr, p.pf_bytes, (int)(blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z)),
+                        (int)(gridDim.x * gridDim.y * gridDim.z), lane - 1, 31);
     }
   } else {
-    // ===== epilogue warps: TMEM lane quadrant = warp % 4
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;  // accumulator row = pixel within the tile
+    // ===== consumer warpgroup wg: pixel rows [64 wg, 64 wg + 64) of the tile
+    const int wg = warp >> 2;
+    float acc[BN / 2];
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+    int stage = 0, prev = -1;
+    uint32_t phase = 0;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait_trap(&full_bar[stage], phase);
+      const uint64_t da = make_wgmma_desc_sw128(smem_u32(smem_a + stage * Cfg::kABytes + wg * 64 * 128));
+      const uint64_t db = make_wgmma_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes));
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k)  // advance 16 elements (32 B) along K inside the 128 B swizzle row: +2 in the (>>4) address field
+        wgmma_f16<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > kb0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();  // the group of the previous stage has retired: its operands may be overwritten
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      prev = stage;
+      if (++stage == Cfg::kStages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) wgmma_fence_operand(acc[j]);
+    named_bar_sync(1, kConsumers);  // both warpgroups are done reading the ring: it becomes the staging tile
+    const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), col0 = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      *reinterpret_cast<float2*>(staging + (size_t)row0 * Cfg::kStageLd + 8 * j + col0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(staging + (size_t)(row0 + 8) * Cfg::kStageLd + 8 * j + col0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+  }
+  __syncthreads();
+  if (p.cluster) cluster_sync_all();  // every CTA of the cluster has staged its partial tile
+
+  if (warp < kConsumers / 32) {
+    // ===== epilogue: thread = (pixel row r, half of the columns this CTA finishes)
+    const int quad = warp & 3, half = warp >> 2;
+    const int r = quad * 32 + lane;
     const int w_off = r % p.TW, h_off = (r / p.TW) % p.TH, n_off = r / (p.TW * p.TH);
     const int n = n0 + n_off, h = h0 + h_off, w = w0 + w_off;
     const bool row_ok = (n < p.NB) && (h < p.H) && (w < p.W);
-    if (p.pf_bytes > 0)
-      l2_prefetch_slice(p.pf_ptr, p.pf_bytes, (int)(blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z)),
-                        (int)(gridDim.x * gridDim.y * gridDim.z), (int)threadIdx.x - 64, 128);
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    const uint32_t taddr_row = tmem_base + ((uint32_t)(quad * 32) << 16);
-    if (p.splits > 1) {
-      // raw fp32 partials -> workspace [split][tile row][Npad]
-      float* ws = p.ws + ((size_t)blockIdx.z * p.ws_rows + (size_t)mt * BM + r) * p.Npad + ncol0;
+    const int S = p.cluster ? p.splits : 1;
+    const int cw = BN / S;  // columns finished by this CTA (a multiple of 16: host)
+    const int c_lo = (p.cluster ? (int)cluster_ctarank() * cw : 0) + half * (cw / 2), c_hi = c_lo + cw / 2;
+    const float* srow = staging + (size_t)r * Cfg::kStageLd;
+    const int64_t o_off = (int64_t)n * p.out_sn + (int64_t)h * p.out_sh + (int64_t)w * p.out_sw;
+    const int64_t r_off = (int64_t)n * p.res_sn + (int64_t)h * p.res_sh + (int64_t)w * p.res_sw;
+    const bool vec_ok = !p.out_f32 && p.out_sc == 1;
+    const bool to_ws = p.splits > 1 && !p.cluster;
+    float* ws = to_ws ? p.ws + ((size_t)blockIdx.z * p.ws_rows + (size_t)mt * BM + r) * p.Npad + ncol0 : nullptr;
 #pragma unroll 1
-      for (int c = 0; c < BN; c += 16) {
-        uint32_t v[16];
-        __syncwarp();
-        tc_ld_32x16(taddr_row + c, v);
-        tc_ld_wait();
-        if (row_ok)  // rows outside the image (partial tiles at the 8x8 / 16x16 levels) are never read back
+    for (int c = c_lo; c < c_hi; c += 8) {
+      float a[8];
+      if (p.cluster) {  // fixed order over the cluster's partial tiles: bit-reproducible
 #pragma unroll
-        for (int j = 0; j < 16; j += 4)
-          *reinterpret_cast<float4*>(ws + c + j) =
-              make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
+        for (int e = 0; e < 8; ++e) a[e] = 0.f;
+        const uint32_t local = smem_u32(srow + c);
+        for (int j = 0; j < S; ++j) {
+          const uint32_t remote = mapa_u32(local, (uint32_t)j);
+          const float4 u0 = ld_cluster_f4(remote), u1 = ld_cluster_f4(remote + 16);
+          a[0] += u0.x; a[1] += u0.y; a[2] += u0.z; a[3] += u0.w;
+          a[4] += u1.x; a[5] += u1.y; a[6] += u1.z; a[7] += u1.w;
+        }
+      } else {
+        const float4 u0 = *reinterpret_cast<const float4*>(srow + c), u1 = *reinterpret_cast<const float4*>(srow + c + 4);
+        a[0] = u0.x; a[1] = u0.y; a[2] = u0.z; a[3] = u0.w;
+        a[4] = u1.x; a[5] = u1.y; a[6] = u1.z; a[7] = u1.w;
       }
-      if (p.fuse_reduce) splitk_fused_reduce<BN>(p, mt, (int)blockIdx.y, (int)gridDim.y, (int)blockIdx.z, r, n, h, w, row_ok, threadIdx.x == 64);
-    } else {
-      const int64_t o_off = (int64_t)n * p.out_sn + (int64_t)h * p.out_sh + (int64_t)w * p.out_sw;
-      const int64_t r_off = (int64_t)n * p.res_sn + (int64_t)h * p.res_sh + (int64_t)w * p.res_sw;
-#pragma unroll 1
-      for (int c = 0; c < BN; c += 16) {
-        uint32_t v[16];
-        __syncwarp();                   // reconverge: the TMEM load is warp-collective (.sync.aligned)
-        tc_ld_32x16(taddr_row + c, v);
-        tc_ld_wait();
-        const int col = ncol0 + c;
-        if (row_ok && col < p.Cout) {
-        float acc[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) acc[j] = __uint_as_float(v[j]);
-        if (col + 16 <= p.Cout && !p.out_f32 && p.out_sc == 1) {
+      if (to_ws) {  // raw fp32 partials -> workspace [split][tile row][Npad]; rows outside the image are never read back
+        if (row_ok) {
+          *reinterpret_cast<float4*>(ws + c) = make_float4(a[0], a[1], a[2], a[3]);
+          *reinterpret_cast<float4*>(ws + c + 4) = make_float4(a[4], a[5], a[6], a[7]);
+        }
+        continue;
+      }
+      const int col = ncol0 + c;
+      float st_s = 0.f, st_q = 0.f;  // flags 2: this row's sum / sum of squares of the octet's fp16 outputs
+      if (row_ok && col < p.Cout) {
+        if (col + 8 <= p.Cout && vec_ok) {
           if (p.bias) {
-#pragma unroll
-            for (int j = 0; j < 16; j += 4) {
-              const float4 b = *reinterpret_cast<const float4*>(p.bias + col + j);
-              acc[j] += b.x; acc[j + 1] += b.y; acc[j + 2] += b.z; acc[j + 3] += b.w;
-            }
+            const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
+            const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + col + 4));
+            a[0] += b0.x; a[1] += b0.y; a[2] += b0.z; a[3] += b0.w;
+            a[4] += b1.x; a[5] += b1.y; a[6] += b1.z; a[7] += b1.w;
           }
           if (p.res) {
-            float rr[16];
+            float rr[8];
             unpack8(ld8(p.res + r_off + col), rr);
-            unpack8(ld8(p.res + r_off + col + 8), rr + 8);
+            if (p.res_mode == 1) {  // CONV flags 4: out = acc * QuickGELU'(u), u = the tile read through the residual path
 #pragma unroll
-            for (int j = 0; j < 16; ++j) acc[j] += rr[j];
+              for (int e = 0; e < 8; ++e) {
+                const float sg = rcp_ftz(1.f + ex2_ftz(-1.702f * 1.4426950408889634f * rr[e]));  // sigmoid(1.702 u), MUFU ex2 + rcp
+                a[e] *= sg * fmaf(1.702f * rr[e], 1.f - sg, 1.f);
+              }
+            } else {
+#pragma unroll
+              for (int e = 0; e < 8; ++e) a[e] += rr[e];
+            }
           }
-          __half* o = reinterpret_cast<__half*>(p.out) + o_off + col;
-          st8(o, pack8(acc));
-          st8(o + 8, pack8(acc + 8));
+          const half8 hv = pack8(a);
+          st8(reinterpret_cast<__half*>(p.out) + o_off + col, hv);
+          if (p.epi_stats) {  // statistics of the ROUNDED values: what the GroupNorm after this conv reads
+            float f[8];
+            unpack8(hv, f);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+              st_s += f[e];
+              st_q = fmaf(f[e], f[e], st_q);
+            }
+          }
         } else {
-          for (int j = 0; j < 16 && col + j < p.Cout; ++j) {
-            float a = acc[j];
-            if (p.bias) a += p.bias[col + j];
-            if (p.res) a += __half2float(p.res[r_off + col + j]);
-            if (p.out_f32) reinterpret_cast<float*>(p.out)[o_off + (col + j) * p.out_sc] = a;
-            else reinterpret_cast<__half*>(p.out)[o_off + (col + j) * p.out_sc] = __float2half_rn(a);
+          for (int e = 0; e < 8 && col + e < p.Cout; ++e) {
+            float x = a[e];
+            if (p.bias) x += p.bias[col + e];
+            if (p.res) x += __half2float(p.res[r_off + col + e]);
+            if (p.out_f32) reinterpret_cast<float*>(p.out)[o_off + (col + e) * p.out_sc] = x;
+            else reinterpret_cast<__half*>(p.out)[o_off + (col + e) * p.out_sc] = __float2half_rn(x);
           }
         }
+      }
+      if (p.epi_stats) {  // 32 rows -> one value per octet and row quarter (warp-uniform branch: full tiles, host)
+        st_s = warp_sum(st_s);
+        st_q = warp_sum(st_q);
+        if (lane == 0) {
+          stat_red[(quad * (BN / 8) + c / 8) * 2] = st_s;
+          stat_red[(quad * (BN / 8) + c / 8) * 2 + 1] = st_q;
         }
       }
     }
+    if (p.epi_stats) {
+      named_bar_sync(1, kConsumers);
+      if ((int)threadIdx.x < BN / 4) {  // thread (octet o = t / 2, kind = t % 2): fixed-order sum over the four row quarters
+        const int o = threadIdx.x >> 1, kind = threadIdx.x & 1, stride = (BN / 8) * 2;
+        const float* src = stat_red + o * 2 + kind;
+        const float v = (src[0] + src[stride]) + (src[2 * stride] + src[3 * stride]);
+        p.epi_stats[((size_t)mt * (p.Npad / 8) + (size_t)(ncol0 / 8 + o)) * 2 + kind] = v;
+      }
+    }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)Cfg::kTmemCols) : "memory");
-  }
+  if (p.cluster) cluster_sync_all();  // the other CTAs' reads of this CTA's staging tile are complete before it exits
 }
 
 // split-K second pass: sum partials, add bias / residual, store.  One thread per 4 consecutive columns (float4 partial
@@ -281,7 +326,7 @@ __global__ void conv_splitk_reduce_kernel(const ConvTcParams p, int m_tiles) {
 
 // ---------------------------------------------------------------- SIMT verification kernel
 // Same contract, CUDA cores only, one thread per output element.  Exists so that GPU tests can
-// cross-check the tcgen05 path layer by layer and so a tcgen05 regression cannot block bring-up of the
+// cross-check the wgmma path layer by layer and so a tensor-core regression cannot block bring-up of the
 // rest of the step; never selected by the shipped plans (impl = 0).
 __global__ void conv_simt_kernel(const __half* __restrict__ A, const __half* __restrict__ Wp, const ConvTcParams p,
                                  int64_t a_sn, int64_t a_sh, int64_t a_sw, int64_t ldb, int64_t b_sh, int64_t b_sn) {
@@ -388,13 +433,10 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
   p.out_sc = op.i[19] > 0 ? op.i[19] : 1;
   if (!p.out_f32 && p.out_sc == 1) CGD_CHECK_ARG(op.i[10] % 8 == 0 && op.i[11] % 8 == 0 && op.i[12] % 8 == 0, "conv: fp16 out strides must be multiples of 8");
   if (p.res) CGD_CHECK_ARG(op.i[13] % 8 == 0 && op.i[14] % 8 == 0 && op.i[15] % 8 == 0 && ((uintptr_t)p.res % 16) == 0, "conv: residual must be 16-byte aligned with strides %% 8 == 0");
-  const bool want_cluster = op.i[23] == 1 && op.i[18] != 1 && op.i[18] != 2;  // plan flag; the SIMT twin / forced single-CTA kernel ignore it
+  const bool want_cluster = op.i[23] == 1 && op.i[18] != 1;  // plan flag; the SIMT twin ignores it
   if (p.splits > 1 && !want_cluster) CGD_CHECK_ARG(p.ws != nullptr, "conv: split-K needs a workspace");
-  L.cluster_split = 0;
-  p.sk_bar = reinterpret_cast<unsigned int*>(op.p[6]);
-  p.epi_stats = nullptr;  // set below for the pair kernel when CONV flags 2 asks for epilogue statistics
-  p.tail_full = 0;        // split last wave (CGD_CONV_TAIL): decided below
-  L.tail_units = 0;
+  p.cluster = 0;
+  p.epi_stats = nullptr;  // set below when CONV flags 2 asks for epilogue statistics
   L.BN = (int)BN;
   L.impl = (int)op.i[18];
   L.A = reinterpret_cast<const __half*>(op.p[0]);
@@ -402,7 +444,7 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
   L.a_sn = op.i[7]; L.a_sh = op.i[8]; L.a_sw = op.i[9];
   L.ldb = op.i[22] > 0 ? op.i[22] : taps * Cin; L.b_sh = op.i[20]; L.b_sn = op.i[21];
   L.m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-  p.ws_rows = ((L.m_tiles + 1) / 2) * 2 * BM;
+  p.ws_rows = L.m_tiles * BM;
   L.n_tiles = (int)(Npad / BN);
   if (L.impl == 1) return 0;
 
@@ -422,129 +464,45 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
   const int64_t ldb = op.i[22] > 0 ? op.i[22] : taps * Cin;
   p.b_batched = (op.i[20] != 0 || op.i[21] != 0) ? 1 : 0;
   CGD_CHECK_ARG(ldb % 8 == 0 && op.i[20] % 8 == 0 && op.i[21] % 8 == 0, "conv: B strides must be multiples of 8 elements");
-  if (p.b_batched) CGD_CHECK_ARG(p.TH == 1 && p.TN == 1 && p.tiles_w % 2 == 0 && L.impl != 2 && L.m_tiles >= 2,
-                                 "conv: batched-B GEMMs need W %% 256 == 0 (one (h, n) per CTA pair) and the pair kernel");
+  if (p.b_batched) CGD_CHECK_ARG(p.TH == 1 && p.TN == 1, "conv: batched-B GEMMs need W > 64 (one (h, n) per 128-pixel tile)");
   {
+    // 4-D map (K, rows, h, n) so batched GEMMs pick their B matrix by the tile's (h, n); plain weights use (0, 0)
     const cuuint64_t K = (cuuint64_t)(taps * Cin);
-    cuuint64_t dims[2] = {K, (cuuint64_t)Npad};
-    cuuint64_t strides[1] = {(cuuint64_t)ldb * 2};
-    cuuint32_t box[2] = {64, (cuuint32_t)BN};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(&L.tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, op.p[1], dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CGD_CHECK_ARG(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled(W) failed with %d", (int)r);
-    // pair kernel: 4-D map (K, rows, h, n) so batched GEMMs pick their B matrix by the tile's (h, n); plain weights use (0, 0)
     const cuuint64_t row_bytes = (cuuint64_t)ldb * 2 * (cuuint64_t)Npad;
     cuuint64_t dims4[4] = {K, (cuuint64_t)Npad, (cuuint64_t)(p.b_batched ? H : 1), (cuuint64_t)(p.b_batched ? NB : 1)};
     cuuint64_t strides4[3] = {(cuuint64_t)ldb * 2, p.b_batched ? (cuuint64_t)op.i[20] * 2 : row_bytes, p.b_batched ? (cuuint64_t)op.i[21] * 2 : row_bytes};
-    cuuint32_t box4[4] = {64, (cuuint32_t)(BN / 2), 1, 1};
+    cuuint32_t box4[4] = {64, (cuuint32_t)BN, 1, 1};
     cuuint32_t estr4[4] = {1, 1, 1, 1};
-    r = enc(&L.tmB2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, op.p[1], dims4, strides4, box4, estr4, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CGD_CHECK_ARG(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled(W half) failed with %d", (int)r);
+    CUresult r = enc(&L.tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, op.p[1], dims4, strides4, box4, estr4, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    CGD_CHECK_ARG(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled(W) failed with %d", (int)r);
   }
   if (want_cluster) {
-    CGD_CHECK_ARG(conv_cluster_split_ok(L), "conv: layer flagged for cluster split-K is not eligible (BN=%d splits=%d Cout=%d f32=%d)", L.BN, p.splits,
-                  p.Cout, p.out_f32);
-    L.cluster_split = 1;
-  }
-  // split-K reduction inside the conv kernel: needs the barrier buffer and every CTA of the launch resident at once
-  {
-    const int64_t units = conv_use_pair_kernel(L) ? (int64_t)((L.m_tiles + 1) / 2) * L.n_tiles * p.splits : (int64_t)L.m_tiles * L.n_tiles * p.splits;
-    p.fuse_reduce = (p.splits > 1 && p.sk_bar != nullptr && units <= (conv_use_pair_kernel(L) ? 74 : 148)) ? 1 : 0;
-    const char* e = getenv("CGD_CONV_FUSE_REDUCE");  // opt-in: see conv_splitk.cuh
-    if (!(e && e[0] == '1')) p.fuse_reduce = 0;
-  }
-  // pair-kernel epilogue through shared memory + TMA tensor stores: same 4-D box geometry as the A operand, so rows outside
-  // the image are clipped by the TMA unit; needs fp16 channel-contiguous output and whole 64-channel chunks
-  p.epi_tma = (!L.cluster_split && conv_use_pair_kernel(L) && !p.out_f32 && p.out_sc == 1 && p.splits == 1 && BN >= 64 && Cout % 64 == 0) ? 1 : 0;
-  if (const char* e = getenv("CGD_CONV_EPI_TMA")) if (e[0] == '0') p.epi_tma = 0;
-  // split last wave (opt-in: CGD_CONV_TAIL=1; device-validated, measured no gain -- DESIGN.md): pair kernel with the TMA-store epilogue, no split-K, tail halves fit a wave
-  L.tail_units = 0;
-  p.tail_full = 0;
-  L.tmB4 = L.tmB2;
-  {
-    static int tail_on = -1;
-    if (tail_on < 0) {
-      const char* e = getenv("CGD_CONV_TAIL");
-      tail_on = (e && e[0] == '1') ? 1 : 0;
-    }
-    const int total = ((L.m_tiles + 1) / 2) * L.n_tiles;
-    if (tail_on && device_sm_count() == 148 && p.epi_tma && !L.cluster_split && !p.b_batched && (BN == 128 || BN == 256) && sched_tail_pays(total, 74)) {
-      const cuuint64_t K = (cuuint64_t)(taps * Cin);
-      const cuuint64_t row_bytes = (cuuint64_t)ldb * 2 * (cuuint64_t)Npad;
-      cuuint64_t dims4[4] = {K, (cuuint64_t)Npad, 1, 1};
-      cuuint64_t strides4[3] = {(cuuint64_t)ldb * 2, row_bytes, row_bytes};
-      cuuint32_t box4[4] = {64, (cuuint32_t)(BN / 4), 1, 1};
-      cuuint32_t estr4[4] = {1, 1, 1, 1};
-      CUresult r = enc(&L.tmB4, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, op.p[1], dims4, strides4, box4, estr4, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      CGD_CHECK_ARG(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled(W quarter) failed with %d", (int)r);
-      p.tail_full = sched_full_tiles(total, 74);
-      L.tail_units = sched_total_units(total, 74);
-    }
-  }
-  // co-resident instantiation of the pair kernel for latency-bound launches (conv_tc2.cu, CO): at most one wave of tiles, or a short
-  // K loop per tile.  Ring depth so that two CTAs fit an SM's 227 KB.  CGD_CONV_CO = 0 | 1 (default off until measured: DESIGN.md).
-  p.nstages = 0;
-  L.co_resident = 0;
-  {
-    static int co_on = -1;
-    if (co_on < 0) {
-      const char* e = getenv("CGD_CONV_CO");
-      co_on = (e && e[0] == '1') ? 1 : 0;
-    }
-    const int64_t units = (int64_t)((L.m_tiles + 1) / 2) * L.n_tiles * p.splits;
-    const int kb_tile = p.kb_per_split > 0 ? p.kb_per_split : p.kblocks;
-    if (co_on && !L.cluster_split && conv_use_pair_kernel(L) && L.tail_units == 0 && !(op.flags & 2) && (units <= 74 || kb_tile <= 16)) {
-      const int stage_bytes = 128 * 64 * 2 + (BN / 2) * 64 * 2;
-      const int fixed = (BN >= 64 ? 2 * 128 * 64 * 2 : 0) + 1024 + 512 + 1024 /* per-CTA reservation */;
-      int ns = ((227 * 1024) / 2 - fixed) / stage_bytes;
-      ns = std::min(ns, 6);
-      if (ns >= 2) {
-        p.nstages = ns;
-        L.co_resident = 1;
-      }
-    }
+    CGD_CHECK_ARG(L.impl != 1 && !p.out_f32 && p.out_sc == 1 && !p.b_batched && p.Cout % 8 == 0 && L.BN >= 64 && p.splits >= 2 && p.splits <= 8 &&
+                      L.BN % p.splits == 0 && (L.BN / p.splits) % 16 == 0,
+                  "conv: layer flagged for cluster split-K is not eligible (BN=%d splits=%d Cout=%d f32=%d)", L.BN, p.splits, p.Cout, p.out_f32);
+    p.cluster = 1;
   }
   // flags 4: the "residual" operand is a QuickGELU pre-activation u and the epilogue computes acc * QuickGELU'(u) instead of acc + res
   p.res_mode = 0;
   if (op.flags & 4) {
-    CGD_CHECK_ARG(p.epi_tma && p.res != nullptr && p.bias == nullptr, "conv: flags 4 (QuickGELU' epilogue) needs the pair kernel's TMA-store epilogue, a res "
-                  "operand and no bias (BN=%d splits=%d Cout=%lld)", BN, p.splits, (long long)Cout);
+    CGD_CHECK_ARG(L.impl != 1 && p.splits == 1 && !p.out_f32 && p.out_sc == 1 && Cout % 8 == 0 && p.res != nullptr && p.bias == nullptr,
+                  "conv: flags 4 (QuickGELU' epilogue) needs the tensor-core kernel without split-K, an fp16 contiguous output with Cout %% 8 == 0, a res "
+                  "operand and no bias (BN=%d splits=%d Cout=%lld)", (int)BN, p.splits, (long long)Cout);
     p.res_mode = 1;
   }
   // flags 2: the epilogue also reduces its output tile to per-octet sums for the GroupNorm that follows (GN_APPLY_EPI): needs the
-  // TMA-store epilogue and tiles that are full and are 128 consecutive pixels of one image
+  // tensor-core kernel without split-K, fp16 contiguous output, and tiles that are full and are 128 consecutive pixels of one image
   p.epi_stats = nullptr;
   if (op.flags & 2) {
-    CGD_CHECK_ARG(p.epi_tma && op.p[7] != nullptr && W % p.TW == 0 && H % p.TH == 0 && p.TN == 1 && (p.TW == W || p.TH == 1) && L.m_tiles % 2 == 0,
-                  "conv: epilogue statistics need the TMA-store epilogue and full 128-pixel tiles inside one image (W=%lld H=%lld tile %dx%dx%d)",
+    CGD_CHECK_ARG(L.impl != 1 && p.splits == 1 && !p.out_f32 && p.out_sc == 1 && op.p[7] != nullptr && W % p.TW == 0 && H % p.TH == 0 && p.TN == 1 &&
+                      (p.TW == W || p.TH == 1),
+                  "conv: epilogue statistics need the tensor-core kernel without split-K, fp16 output and full 128-pixel tiles inside one image (W=%lld H=%lld tile %dx%dx%d)",
                   (long long)W, (long long)H, p.TW, p.TH, p.TN);
     p.epi_stats = reinterpret_cast<float*>(op.p[7]);
   }
-  if (p.epi_tma) {
-    cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)NB};
-    cuuint32_t box[4] = {64, (cuuint32_t)p.TW, (cuuint32_t)p.TH, (cuuint32_t)p.TN};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    cuuint64_t ostr[3] = {(cuuint64_t)p.out_sw * 2, (cuuint64_t)p.out_sh * 2, (cuuint64_t)p.out_sn * 2};
-    CUresult r = enc(&L.tmOut, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, p.out, dims, ostr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CGD_CHECK_ARG(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled(out) failed with %d", (int)r);
-    if (p.res) {
-      cuuint64_t rstr[3] = {(cuuint64_t)p.res_sw * 2, (cuuint64_t)p.res_sh * 2, (cuuint64_t)p.res_sn * 2};
-      r = enc(&L.tmRes, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)p.res, dims, rstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      CGD_CHECK_ARG(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled(res) failed with %d", (int)r);
-    } else {
-      L.tmRes = L.tmOut;
-    }
-  } else {
-    L.tmOut = L.tmA;  // unused, but kernel parameters must be valid descriptors
-    L.tmRes = L.tmA;
-  }
   // <= 8 output channels, fp32 output, 3x3 (UNet head, stem dgrad): halo-tile mma.sync kernel (conv_narrow.cu); CGD_CONV_NARROW=0 keeps
-  // the tcgen05 N = 16 tile for A/B runs
+  // the wgmma N = 16 tile for A/B runs
   {
     static int narrow_on = -1;
     if (narrow_on < 0) {
@@ -554,8 +512,8 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
     L.narrow = (narrow_on && conv_narrow_eligible(L)) ? 1 : 0;
   }
   // 8 x 8 images (deepest UNet level): one launch, a CTA per 8 output channels streaming its whole weight slab (conv_narrow.cu,
-  // conv_small_kernel) instead of split-K tiles + a reduce launch.  Opt-in (CGD_CONV_SMALL=1): device-validated, but measured
-  // break-even per launch (17.7 vs 18.6 us for the 1024 -> 1024 3x3) and -0.5 % in the step (profiles/r02_call_s_small_v3.log).
+  // conv_small_kernel) instead of split-K tiles + a reduce launch.  Opt-in (CGD_CONV_SMALL=1): not measured against the wgmma
+  // split-K path on the H100.
   {
     static int small_on = -1;
     if (small_on < 0) {
@@ -579,26 +537,86 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
 }
 
 template <int BN>
-static int launch_tc(const ConvTcLaunch& L, cudaStream_t st) {
-  using Cfg = TcCfg<BN>;
+static int set_smem_attr() {
   static DeviceOnce attr_set;
   if (attr_set.needed()) {
-    CGD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    CGD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BN>::kSmemBytes));
     attr_set.mark();
   }
-  dim3 grid(L.m_tiles, L.n_tiles, L.p.splits);
-  CGD_CUDA(launch_pdl(conv_tc_kernel<BN>, grid, dim3(kThreads), Cfg::kSmemBytes, st, L.tmA, L.tmB, L.p));
   return 0;
 }
 
-// impl: 0 = auto (CTA-pair persistent kernel when the layer has at least two 128-pixel tiles, else the single-CTA kernel),
-// 1 = SIMT verification twin, 2 = force single-CTA kernel, 3 = force CTA-pair kernel
-bool conv_use_pair_kernel(const ConvTcLaunch& L) { return L.impl == 3 || (L.impl == 0 && L.m_tiles >= 2); }
+template <int BN>
+static int launch_tc(const ConvTcLaunch& L, cudaStream_t st) {
+  using Cfg = TcCfg<BN>;
+  if (const int rc = set_smem_attr<BN>()) return rc;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)L.m_tiles, (unsigned)L.n_tiles, (unsigned)L.p.splits);
+  cfg.blockDim = dim3(kThreads);
+  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
+  cfg.stream = st;
+  cudaLaunchAttribute attrs[2];
+  int na = 0;
+  if (L.p.cluster) {  // the `splits` CTAs of one output tile form a cluster along z
+    attrs[na].id = cudaLaunchAttributeClusterDimension;
+    attrs[na].val.clusterDim.x = 1;
+    attrs[na].val.clusterDim.y = 1;
+    attrs[na].val.clusterDim.z = (unsigned)L.p.splits;
+    ++na;
+  }
+  if (pdl_enabled()) {
+    attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attrs[na].val.programmaticStreamSerializationAllowed = 1;
+    ++na;
+  }
+  cfg.attrs = attrs;
+  cfg.numAttrs = na;
+  CGD_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN>, L.tmA, L.tmB, L.p));
+  return 0;
+}
 
+template <int BN>
+static int max_clusters(int S) {
+  if (set_smem_attr<BN>() != 0) {
+    cudaGetLastError();
+    return -1;
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(64, 1, (unsigned)S);
+  cfg.blockDim = dim3(kThreads);
+  cfg.dynamicSmemBytes = TcCfg<BN>::kSmemBytes;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = 1;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = (unsigned)S;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  int n = 0;
+  if (cudaOccupancyMaxActiveClusters(&n, conv_tc_kernel<BN>, &cfg) != cudaSuccess) {
+    cudaGetLastError();
+    return -1;
+  }
+  return n;
+}
+// co-resident clusters of S CTAs the device can hold for tile width BN (cudaOccupancyMaxActiveClusters); -1 without a device
+int conv_cluster_capacity(int BN, int S) {
+  if (S < 1 || S > 8) return -1;
+  switch (BN) {
+    case 64: return max_clusters<64>(S);
+    case 128: return max_clusters<128>(S);
+    case 192: return max_clusters<192>(S);
+    case 256: return max_clusters<256>(S);
+    default: return -1;
+  }
+}
+
+// impl: 0 = auto, 1 = SIMT verification twin, 2 / 3 = the wgmma tile kernel for every layer (no narrow / 8 x 8 special kernels;
+// the plan uses in-cluster split-K and the fused epilogues with 0 and 3 only)
 int conv_tc_launch(const ConvTcLaunch& L, cudaStream_t st) {
   if (L.impl == 1) {
     const int64_t total = (int64_t)L.p.NB * L.p.H * L.p.W * L.p.Cout;
-    const int blocks = (int)std::min<int64_t>(ceil_div(total, 256), 148 * 16);
+    const int blocks = (int)std::min<int64_t>(ceil_div(total, 256), (int64_t)device_sm_count() * 16);
     ConvTcParams p = L.p;
     p.splits = 1;
     CGD_CUDA(launch_pdl(conv_simt_kernel, dim3(blocks), dim3(256), 0, st, L.A, L.Wp, p, L.a_sn, L.a_sh, L.a_sw, L.ldb, L.b_sh, L.b_sn));
@@ -606,11 +624,7 @@ int conv_tc_launch(const ConvTcLaunch& L, cudaStream_t st) {
   }
   if (L.narrow) return conv_narrow_launch(L, st);
   if (L.small) return conv_small_launch(L, st);
-  if (L.cluster_split) return conv_tc3_launch(L, st);
   int rc = 0;
-  if (conv_use_pair_kernel(L)) rc = conv_tc2_launch(L, st);
-  else if (L.p.b_batched) { set_error("conv: batched-B GEMM reached the single-CTA kernel"); return -1; }
-  else
   switch (L.BN) {
     case 16: rc = launch_tc<16>(L, st); break;
     case 32: rc = launch_tc<32>(L, st); break;
@@ -621,16 +635,16 @@ int conv_tc_launch(const ConvTcLaunch& L, cudaStream_t st) {
     default: set_error("conv: unsupported BN %d", L.BN); return -1;
   }
   if (rc) return rc;
-  if (L.p.splits > 1 && !L.p.fuse_reduce) {
+  if (L.p.splits > 1 && !L.p.cluster) {
     const int64_t total = (int64_t)L.m_tiles * BM * ((L.p.Cout + 3) / 4);
-    const int blocks = (int)std::min<int64_t>(ceil_div(total, 256), 148 * 8);
+    const int blocks = (int)std::min<int64_t>(ceil_div(total, 256), (int64_t)device_sm_count() * 8);
     CGD_CUDA(launch_pdl(conv_splitk_reduce_kernel, dim3(blocks), dim3(256), 0, st, L.p, L.m_tiles));
   }
   return 0;
 }
 
 int conv_tc_num_launches(const ConvTcLaunch& L) {
-  return (L.impl != 1 && !L.small && !L.narrow && L.p.splits > 1 && !L.p.fuse_reduce && !L.cluster_split) ? 2 : 1;
+  return (L.impl != 1 && !L.small && !L.narrow && L.p.splits > 1 && !L.p.cluster) ? 2 : 1;
 }
 
 }  // namespace cgd

@@ -1,4 +1,4 @@
-// conv_tc.cuh -- parameter blocks of the tcgen05 implicit-GEMM conv (see conv_tc.cu).
+// conv_tc.cuh -- parameter blocks of the wgmma implicit-GEMM conv (see conv_tc.cu).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -15,13 +15,10 @@ struct ConvTcParams {
   int kblocks, splits, kb_per_split; // K loop = taps * Cin/64 blocks, optionally split over gridDim.z
   int out_f32;
   int b_batched;                     // B operand indexed by the tile's (h, n) (batched GEMM: attention)
-  int ws_rows;                       // rows per split in the split-K workspace (= even-rounded m_tiles * 128)
-  int epi_tma;                       // pair kernel: outputs leave through shared memory + TMA tensor stores (fp16, Cout % 64 == 0)
-  unsigned int* sk_bar;              // split-K: 2 u32 per (128-pixel tile, channel tile), see conv_splitk.cuh
-  int fuse_reduce;                   // split-K partials are reduced by the conv kernel itself (all CTAs of the launch co-resident)
-  const void* pf_ptr;                // next conv's packed weights: prefetched into L2 by the idle epilogue warps (0 = none)
+  int ws_rows;                       // rows per split in the split-K workspace (= m_tiles * 128)
+  int cluster;                       // split-K inside a cluster of `splits` CTAs along z, reduced through distributed shared memory
+  const void* pf_ptr;                // next conv's packed weights: prefetched into L2 by the idle lanes of the TMA warp (0 = none)
   int64_t pf_bytes;
-  int dbg;                           // CGD_CONV_DBG (profiling experiments only): 1 = no TMA loads, 2 = no MMAs, 4 = no epilogue stores
   int64_t out_sn, out_sh, out_sw;    // output / residual strides in elements (channel contiguous)
   int64_t res_sn, res_sh, res_sw;
   int64_t out_sc;                    // output channel stride (1 except for NCHW fp32 outputs; scalar-store paths only)
@@ -29,27 +26,18 @@ struct ConvTcParams {
   const __half* res;
   void* out;
   float* ws;                         // split-K partials [splits][m_tiles*128][Npad]
-  int tail_full;                     // pair kernel, TAIL instantiation: tiles kept whole (conv_sched.cuh); the rest is split in halves
-  int res_mode;                      // pair kernel, TMA-store epilogue: 0 = out = acc (+bias) + res ; 1 = out = acc * QuickGELU'(res) (CONV flags 4:
-                                     // the dgrad of the ViT's c_proj writes d(c_fc output) directly, `res` = the saved pre-activation)
-  int nstages;                       // pair kernel: operand-ring depth of this launch (<= Tc2Cfg::kStages); fewer stages = less shared memory, so that
-                                     // the next kernel's CTAs can become resident (programmatic dependent launch) while this one drains
+  int res_mode;                      // 0 = out = acc (+bias) + res ; 1 = out = acc * QuickGELU'(res) (CONV flags 4: the dgrad of the ViT's
+                                     // c_proj writes d(c_fc output) directly, `res` = the saved pre-activation)
   float* epi_stats;                  // flags 2: per (128-pixel tile, 8-channel octet) sum / sum of squares of the fp16 OUTPUT, [m_tiles][Npad/8][2]
 };
 
 struct ConvTcLaunch {
-  CUtensorMap tmA, tmB;              // A: 4-D pixel box; B: [BN x 64] weight slice (single-CTA kernel)
-  CUtensorMap tmB2;                  // B: [BN/2 x 64] half slice per CTA of a pair (cta_group::2 kernel)
-  CUtensorMap tmOut, tmRes;          // pair kernel epilogue: [64 ch x TW x TH x TN] boxes of the output / residual
+  CUtensorMap tmA, tmB;              // A: 4-D pixel box; B: 4-D (K, rows, h, n) map, [BN x 64] weight slice per load
   CUtensorMap tmS;                   // 8 x 8 images (conv_small_kernel): the whole image + zero border as one [64 ch x 10 x 10 x 1] box (3x3) / [64 x 8 x 8 x 1] (1x1)
-  CUtensorMap tmB4;                  // B: [BN/4 x 64] quarter slice per CTA (half tiles of the split last wave)
-  int tail_units;                    // > 0: launch the TAIL instantiation over this many schedule units
   ConvTcParams p;
   int BN, impl, m_tiles, n_tiles;
   int small;                         // 8 x 8 images: the weight-streaming mma.sync kernel of conv_narrow.cu (8 output channels per CTA, no split-K)
-  int narrow;                        // <= 8 output channels, fp32 out, 3x3: the halo-tile mma.sync kernel of conv_narrow.cu instead of a tcgen05 tile
-  int co_resident;                   // pair kernel: launch the 2-CTAs-per-SM instantiation with a short operand ring (latency-bound layers)
-  int cluster_split;                 // split-K inside a 2*splits-CTA cluster, reduced through DSMEM (conv_tc3.cu): no workspace, one launch
+  int narrow;                        // <= 8 output channels, fp32 out, 3x3: the halo-tile mma.sync kernel of conv_narrow.cu instead of a wgmma tile
   const __half* A;
   const __half* Wp;
   int64_t a_sn, a_sh, a_sw;
@@ -59,14 +47,10 @@ struct ConvTcLaunch {
 int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L);
 int conv_tc_launch(const ConvTcLaunch& L, cudaStream_t st);
 int conv_tc_num_launches(const ConvTcLaunch& L);
-int conv_tc2_launch(const ConvTcLaunch& L, cudaStream_t st);  // conv_tc2.cu
-bool conv_use_pair_kernel(const ConvTcLaunch& L);
-int conv_tc3_launch(const ConvTcLaunch& L, cudaStream_t st);  // conv_tc3.cu
 bool conv_narrow_eligible(const ConvTcLaunch& L);              // conv_narrow.cu
 int conv_narrow_launch(const ConvTcLaunch& L, cudaStream_t st);
 bool conv_small_eligible(const ConvTcLaunch& L);
 int conv_small_launch(const ConvTcLaunch& L, cudaStream_t st);
-bool conv_cluster_split_ok(const ConvTcLaunch& L);
-int conv_tc3_max_clusters(int BN, int S);
+int conv_cluster_capacity(int BN, int S);
 
 }  // namespace cgd

@@ -2,7 +2,7 @@
 //
 // The HBM-bound glue of the [3P] UNet / ViT graphs that the reference issues as many small ATen launches
 // (SURVEY.md K6, K7, K8, K15): 128-bit vectorised, coalesced along channels, grid-stride loops sized to a
-// multiple of the 148 SMs.
+// multiple of the 132 SMs.
 #include "common.cuh"
 #include "pdl.cuh"
 #include "ops.cuh"
@@ -11,15 +11,14 @@ namespace cgd {
 
 static inline int ew_blocks(int64_t work_items, int threads = 256) {
   int64_t b = ceil_div(work_items, threads);
-  const int64_t cap = 148 * 8;
+  const int64_t cap = 132 * 8;
   if (b > cap) b = cap;
   if (b < 1) b = 1;
   return (int)b;
 }
 
 // Index arithmetic: these kernels decode a flat index into (n, y, x, vector).  With int64 operands every / and % is a ~100-instruction
-// software routine and the decode, not the memory system, bounded them (profiles/r02_launches_v1_warm.csv: UP2 128x128 -> 256x256 x 256
-// 16.6 us for 42 MB = 2.5 TB/s where ADD moves 100 MB at 6.3 TB/s).  IdxT = uint32_t whenever the element count allows (always, here).
+// software routine and the decode, not the memory system, would bound them.  IdxT = uint32_t whenever the element count allows (always, here).
 // ---- 2x2 pooling (sum * scale) on pixel-major [N,H,W,C]
 template <typename IdxT>
 __global__ void pool2_kernel(const __half* __restrict__ x, __half* __restrict__ y, int N, int H, int W, int C, int64_t ldx,
@@ -112,7 +111,7 @@ int launch_pool2(const CgdOp& op, cudaStream_t st) {
   const int64_t N = op.i[0], H = op.i[1], W = op.i[2], C = op.i[3], ldx = op.i[4], ldy = op.i[5];
   CGD_CHECK_ARG(N > 0 && H % 2 == 0 && W % 2 == 0 && C % 8 == 0 && ldx % 8 == 0 && ldy % 8 == 0 && op.p[0] && op.p[1], "pool2: bad args");
   const int64_t items = N * (H / 2) * (W / 2) * (C / 8);
-  if (items + (int64_t)148 * 8 * 256 < (int64_t(1) << 32))
+  if (items + (int64_t)132 * 8 * 256 < (int64_t(1) << 32))
     CGD_CUDA(launch_pdl(pool2_kernel<uint32_t>, dim3(ew_blocks(items)), dim3(256), 0, st, (const __half*)op.p[0], (__half*)op.p[1], (int)N, (int)H, (int)W,
                         (int)C, ldx, ldy, op.f[0]));
   else
@@ -125,7 +124,7 @@ int launch_up2(const CgdOp& op, cudaStream_t st) {
   const int64_t N = op.i[0], H = op.i[1], W = op.i[2], C = op.i[3], ldx = op.i[4], ldy = op.i[5];
   CGD_CHECK_ARG(N > 0 && H > 0 && W > 0 && C % 8 == 0 && ldx % 8 == 0 && ldy % 8 == 0 && op.p[0] && op.p[1], "up2: bad args");
   const int64_t items = N * H * W * (C / 8);  // one thread per input vector
-  if (items + (int64_t)148 * 8 * 256 < (int64_t(1) << 32))
+  if (items + (int64_t)132 * 8 * 256 < (int64_t(1) << 32))
     CGD_CUDA(launch_pdl(up2_kernel<uint32_t>, dim3(ew_blocks(items)), dim3(256), 0, st, (const __half*)op.p[0], (__half*)op.p[1], (int)N, (int)H, (int)W, (int)C,
                         ldx, ldy, op.f[0]));
   else

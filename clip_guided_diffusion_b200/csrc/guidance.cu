@@ -17,14 +17,13 @@ namespace cgd {
 
 static inline int gw_blocks(int64_t items, int threads = 256) {
   int64_t b = ceil_div(items, threads);
-  if (b > 148 * 8) b = 148 * 8;
+  if (b > 132 * 8) b = 132 * 8;
   if (b < 1) b = 1;
   return (int)b;
 }
 
 // adaptive_avg_pool2d bin of output index o for input extent S -> [start, end)
-// (32-bit arithmetic: o < cs <= 1024 and S <= 16384 keep every product below 2^31; the 64-bit divisions this replaces made the
-// backward gather 175 us)
+// (32-bit arithmetic: o < cs <= 1024 and S <= 16384 keep every product below 2^31; 64-bit divisions are software routines)
 __device__ __forceinline__ void pool_bin(int o, int S, int cs, int& s, int& e) {
   s = (int)(((unsigned)o * (unsigned)S) / (unsigned)cs);
   e = (int)((((unsigned)(o + 1)) * (unsigned)S + (unsigned)cs - 1u) / (unsigned)cs);
@@ -111,7 +110,7 @@ __global__ void cutouts_bwd_kernel(const __half* __restrict__ dpatch, const int*
 
 // ---------------------------------------------------------------- cutouts, row-per-warp version (default)
 // The element-per-thread kernels above decode (row, patch, c, ky, kx) with div / mod chains and recompute both pooling bins for
-// every element: 43 us forward / 108 us backward at cfg2 for ~15 MB of (mostly L2-resident) traffic.  Here the bin tables are built
+// every element, which makes them issue-bound on ~15 MB of (mostly L2-resident) traffic at cfg2.  Here the bin tables are built
 // once per block in shared memory, a warp owns one output row (forward) or one image row (backward), lanes walk consecutive x --
 // coalesced reads of the source row(s), contiguous fp16 writes per patch row -- and nothing is divided in the inner loops.
 // Same sums in the same order as the kernels above; the bin mean / normalisation use reciprocals instead of IEEE divisions (<= 1 fp32

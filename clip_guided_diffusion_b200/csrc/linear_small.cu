@@ -95,7 +95,7 @@ int launch_linear_small(const CgdOp& op, cudaStream_t st) {
   CGD_CHECK_ARG((size_t)LS_MT * K * sizeof(float) <= 96 * 1024, "linear_small: K=%lld too large", (long long)K);
   const int smem = (int)(LS_MT * K * sizeof(float));
   const int silu = op.flags & 1, acc = (op.flags & 2) ? 1 : 0, xh = (op.flags & 4) ? 1 : 0, yh = (op.flags & 8) ? 1 : 0, wh = (op.flags & 16) ? 1 : 0;
-  const dim3 grid((unsigned)std::min<int64_t>(ceil_div(N, 8), 148 * 4), (unsigned)ceil_div(M, LS_MT));
+  const dim3 grid((unsigned)std::min<int64_t>(ceil_div(N, 8), 132 * 4), (unsigned)ceil_div(M, LS_MT));
   if (xh && wh) return ls_launch<__half, __half>(op, st, grid, smem, (int)M, (int)K, (int)N, ldx, ldy, silu, acc, yh);
   if (xh) return ls_launch<__half, float>(op, st, grid, smem, (int)M, (int)K, (int)N, ldx, ldy, silu, acc, yh);
   if (wh) return ls_launch<float, __half>(op, st, grid, smem, (int)M, (int)K, (int)N, ldx, ldy, silu, acc, yh);

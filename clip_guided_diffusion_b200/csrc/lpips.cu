@@ -1,6 +1,6 @@
 // lpips.cu -- the non-conv pieces of the LPIPS-VGG16 perceptual loss and its input gradient ([3P] lpips.LPIPS(net='vgg'), used by
 // the reference when an init image is given: cgd/cgd.py:147-148, 220-224; SURVEY.md A.4, K21).  The 13 conv3x3 layers run on the
-// tcgen05 conv kernel (conv_tc2.cu); here: ReLU, 2x2 max-pool, and the per-tap "unit-normalise over channels, squared difference
+// wgmma conv kernel (conv_tc.cu); here: ReLU, 2x2 max-pool, and the per-tap "unit-normalise over channels, squared difference
 // to the (precomputed, normalised) init-image features, 1x1 lin, spatial mean" with its analytic gradient.  All HBM-bound
 // elementwise / per-pixel kernels on pixel-major fp16 activations, 128-bit accesses.
 #include "common.cuh"
@@ -11,7 +11,7 @@ namespace cgd {
 
 static inline int lp_blocks(int64_t n, int per_block = 256) {
   int64_t b = (n + per_block - 1) / per_block;
-  if (b > 148 * 8) b = 148 * 8;
+  if (b > 132 * 8) b = 132 * 8;
   return (int)(b < 1 ? 1 : b);
 }
 

@@ -343,7 +343,7 @@ static int gn_check(const CgdOp& op, int64_t C, int64_t HW, int64_t N) {
 }
 static int gn_apply_chunks(int64_t HW, int64_t N, int PP) {
   int64_t c = ceil_div(HW, (int64_t)PP * 8);
-  const int64_t cap = ceil_div(148 * 3, N);
+  const int64_t cap = ceil_div(132 * 3, N);
   if (c > cap) c = cap;
   if (c < 1) c = 1;
   return (int)c;

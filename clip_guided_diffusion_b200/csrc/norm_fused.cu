@@ -1,9 +1,8 @@
 // norm_fused.cu -- single-launch GroupNorm(32) (+SiLU, +scale/shift) forward and input-gradient for activations whose
 // per-(image, group) slab fits the registers of one thread-block cluster.
 //
-// Why (measured, profiles/r01_launches_cfg2_step_v3.csv): the two-pass kernels of norm.cu cost 13 + 8 us (forward) and
-// 20 + 10 us (backward) per layer *independently of size* at the 8x8 .. 64x64 levels of the UNet -- a chain of
-// load -> block reduce -> partials -> fence -> atomic -> last-block fold -> second launch -> reload -- while the data is
+// Why: the two-pass kernels of norm.cu cost two launches per layer *independently of size* at the 8x8 .. 64x64 levels of the
+// UNet -- a chain of load -> block reduce -> partials -> fence -> atomic -> last-block fold -> second launch -> reload -- while the data is
 // 0.1 .. 8 MB.  Here one cluster of CS CTAs owns `gpc` consecutive groups of one image: the slab is read ONCE into
 // registers, statistics are exact two-pass (mean, then sum (x - mean)^2) and are exchanged between the CTAs of the cluster
 // through distributed shared memory in a fixed order (deterministic), then the slab is normalised from registers and written.

@@ -1,16 +1,16 @@
 // norm_grid.cu -- GroupNorm(32) (+SiLU, +scale/shift) forward and input-gradient for LARGE activations as ONE persistent
 // launch: statistics pass, grid-wide barrier, apply pass, both passes fed by a bulk-async-copy (TMA) ring.
 //
-// Why (measured on B200, profiles/r01_gn_microbench_v1/v2.txt): at the 128x128 / 256x256 levels the two-launch kernels of
-// norm.cu reach 0.9 - 1.7 TB/s of the 6.5 TB/s copy bandwidth (two blocks of 256 threads per SM keep ~5 MB in flight, the grids
-// end in half-empty waves, the second launch waits for a last-block fold), and a first single-launch version whose threads
-// loaded 8 x 16 B each stopped at 2 TB/s: the bytes in flight were bounded by registers.  Here one CTA per SM owns a
+// Why: at the 128x128 / 256x256 levels the two-launch kernels of
+// norm.cu keep too few bytes in flight (two blocks of 256 threads per SM), their grids end in half-empty waves and the second
+// launch waits for a last-block fold; a single-launch version whose threads load a few 16-byte vectors each is bounded by the
+// registers that hold the bytes in flight.  Here one CTA per SM owns a
 // contiguous pixel range of one image across ALL channels; a producer warp streams it through an 8-stage shared-memory
-// ring with cp.async.bulk (16 KB per stage, 128 KB in flight per SM = 19 MB over the chip, independent of the consumers'
+// ring with cp.async.bulk (16 KB per stage, 128 KB in flight per SM, independent of the consumers'
 // registers); 512 consumer threads reduce each stage from shared memory, write per-group partial sums, meet the other CTAs
 // at a generation-counted grid barrier (every CTA is resident: grid <= SM count, one CTA per SM), fold the partials
 // themselves (fixed order, compensated fp32: bit-identical in every CTA) and normalise the same pixel range from a second trip through
-// the ring, whose loads are L2 hits (the tensors are 8 - 67 MB, the L2 is 126 MB) and start while the barrier is still
+// the ring, whose loads are largely L2 hits (the tensors are 8 - 67 MB, the L2 is 50 MB) and start while the barrier is still
 // being crossed.  HBM traffic: x once + y once (forward), dy + x once + dx (backward).
 //
 // Replaces [3P] guided-diffusion GroupNorm32 + SiLU + scale-shift and their autograd (SURVEY.md K5, K6).
@@ -74,8 +74,7 @@ __device__ __forceinline__ void gng_block_reduce(const float* s, const float* q,
 
 // Fold the Gn per-CTA partials of image n (layout [Gn][32][2]) in a fixed order: thread (g, part) takes CTAs part, part+16, ...
 // with Neumaier-compensated fp32 sums (exact to ~1 ulp for <= 10 terms), the 16 parts are folded by shuffles.  No fp64: the
-// F2F.F64 / DADD sequence of the first version was 10 % of the kernel's stall samples (B200's fp64 pipe is narrow) for a
-// reduction of 148 numbers.  Results for all 32 groups land in shared memory.
+// F2F.F64 / DADD sequence of a double-precision fold stalls on the narrow fp64 pipe for a reduction of one number per SM.  Results for all 32 groups land in shared memory.
 __device__ __forceinline__ void gng_fold(const float* part_n, int Gn, float* out_a, float* out_b) {
   const int g = threadIdx.x >> 4, part = threadIdx.x & 15;
   float sa = 0.f, ca = 0.f, sb = 0.f, cb = 0.f;
@@ -439,10 +438,9 @@ bool gn_stream_supports(int64_t C);
 int gn_stream_partial_floats(int64_t N, int64_t HW, int64_t C);
 int launch_gn_fwd_stream(const CgdOp& op, cudaStream_t st);
 int launch_gn_bwd_stream(const CgdOp& op, cudaStream_t st);
-// Engines behind GN_FWD_GRID / GN_BWD_GRID.  Measured: persistent ring vs persistent direct (profiles/r01_gn_microbench_v4.txt): direct
-// wins the backward of the 256x256 level (51 vs 57 us at C = 256, 86 vs 104 us at C = 512), ties at 128x128 x 512, loses 3 - 5 us
-// elsewhere.  Both are schedule-bound, not traffic-bound (profiles/r02_launches_v1*: the one-trip GN_APPLY_EPI took as long as the
-// two-trip kernel); the streaming engine (three launches, norm_stream.cu) is the attempt at that, opt-in until it measures faster
+// Engines behind GN_FWD_GRID / GN_BWD_GRID: persistent ring, persistent direct (used for the large backward launches, where it keeps
+// more bytes in flight), and the streaming engine (three launches, norm_stream.cu), opt-in; none of the three has been compared on
+// the H100
 // (needs C % 256 == 0 and room in the op's partials buffer: i6 forward / i7 backward = capacity in floats).
 // CGD_GN_GRID_ENGINE = ring | direct | stream forces one engine for A/B runs.
 enum { kEngRing = 0, kEngDirect = 1, kEngStream = 2 };

@@ -2,15 +2,11 @@
 // the single persistent launch of norm_grid.cu: same contract (ops GN_FWD_GRID / GN_BWD_GRID, same partials / barrier / stats
 // buffers), different engine.
 //
-// What the first version measured (ncu, profiles/r01_gn_grid_256_v1_ncu_raw.csv, 256x256x256): 13.3 M warp instructions for
-// 16.7 M elements (25 thread instructions per element), issue slots 39 % busy at 16 consumer warps per SM, DRAM 11 % of
-// peak -- a latency-bound instruction stream, not a memory-bound one: one 16-byte vector per loop trip with a serial
+// Why: the ring kernel's consumers are a latency-bound instruction stream, not a memory-bound one: one 16-byte vector per loop trip with a serial
 // HADD2 -> FFMA -> FMUL -> MUFU.EX2 -> FADD -> MUFU.RCP -> FMUL -> F2FP -> STG chain (85 SASS instructions per vector in
 // the apply trip), generic-address LD from the shared-memory ring, mbarrier spin loops in every consumer warp.
-// Here: 1024 threads per SM (32 warps) read global memory directly (the tensors are L2-resident: 8 - 67 MB in a 126 MB L2, the
-// statistics trip pulls what is not), every thread owns ONE 8-channel column for the whole kernel, so the per-channel
-// coefficients live in registers, U vectors are in flight per thread per trip (U x 16 KB per SM), and the arithmetic uses the
-// packed fp32 pair instructions (FFMA2 / FMUL2 / FADD2): 44 instead of 68 arithmetic instructions per vector.
+// Here: 1024 threads per SM (32 warps) read global memory directly (the second trip finds much of the 8 - 67 MB tensor in the 50 MB L2), every thread owns ONE 8-channel column for the whole kernel, so the per-channel
+// coefficients live in registers, and U vectors are in flight per thread per trip (U x 16 KB per SM).
 // Requires C % 256 == 0 (a thread's 8 channels never straddle a group); other widths keep the ring kernels.
 //
 // Replaces [3P] guided-diffusion GroupNorm32 + SiLU + scale-shift and their autograd (SURVEY.md K5, K6).
@@ -214,7 +210,7 @@ gn_fwd_grid2_kernel(const __half* __restrict__ x, const float* __restrict__ gamm
 
 // ------------------------------------------------------------------------------------------------ forward from conv-epilogue statistics
 // GN_APPLY_EPI: the conv that produced x already reduced it to per (128-pixel tile, 8-channel octet) sums (CONV flags 2,
-// conv_tc2.cu STATS), so the forward is ONE streaming trip: every CTA folds the partial sums of its image (warp g = group g, fixed
+// conv_tc.cu, CONV flags 2), so the forward is ONE streaming trip: every CTA folds the partial sums of its image (warp g = group g, fixed
 // order, compensated fp32 -- bit-identical in every CTA, no grid barrier), then applies.  partials: [N * tpi][octs][2], tpi = HW / 128.
 template <int U>
 __global__ void __launch_bounds__(kG2Threads, 1)

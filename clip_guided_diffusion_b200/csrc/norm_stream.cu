@@ -3,10 +3,8 @@
 //
 // Why: the persistent one-launch kernels (norm_grid.cu ring, norm_grid2.cu direct) run ONE 544- / 1024-thread CTA per SM whose
 // threads move in lock-step through load -> compute phases, with a software grid barrier and a per-CTA fold between the two trips.
-// Measured in the step (profiles/r02_launches_v1_warm.csv): 35.8 us for 67 MB at 256x256x256 (1.9 TB/s) -- and the one-trip
-// GN_APPLY_EPI variant, which skips the whole statistics trip, still took 34.1 us: the time is not the traffic, it is the
-// lock-step schedule at 25 - 50 % occupancy.  The elementwise kernels of this library (elementwise.cu: 256-thread CTAs, 8 per SM,
-// grid-stride, one 16-byte vector per trip) move the same tensors at 6.3 TB/s (ADD: 100 MB in 15.8 us).  So: the same shape here.
+// That schedule, at 25 - 50 % occupancy, rather than the traffic can bound them; the elementwise kernels of this library
+// (elementwise.cu: 256-thread CTAs, 8 per SM, grid-stride, one 16-byte vector per trip) are shaped for streaming, so: the same shape here.
 //   forward :  [gn_stats_stream | conv-epilogue partials]  ->  gn_fold  ->  gn_apply_stream
 //   backward:   gn_bwd_stats_stream                        ->  gn_fold  ->  gn_bwd_apply_stream
 // Three short launches (PDL-chained) instead of one persistent one; every thread owns one 8-channel column for the whole kernel
@@ -22,7 +20,7 @@
 namespace cgd {
 
 constexpr int kGsThreads = 256;
-constexpr int kGsMaxCtas = 148 * 8;  // partial slots per launch (plan.py allocates N * kGsMaxCtas * 64 floats at most)
+constexpr int kGsMaxCtas = 132 * 8;  // partial slots per launch (plan.py allocates N * kGsMaxCtas * 64 floats at most)
 
 __device__ __forceinline__ uint4 gs_ld(const __half* p) {
   uint4 v;
@@ -99,9 +97,8 @@ __device__ __forceinline__ void gs_block_partials(const GsMap& m, int vpg, float
 // ------------------------------------------------------------------------------------------------ fold
 // sums[n][g][2] = sum over the partials of image n, group g.  mode 0: partials [n][G][32][2] (one row per CTA of a *_stats_stream
 // launch); mode 1: conv-epilogue partials [n * tpi + tile][octs][2] (CONV flags 2), group g = octets [oct0 + g * vpg, + vpg) of each
-// of the image's tpi tiles.  grid (32 groups, N), 256 threads: every thread takes a few partials with INDEPENDENT loads (a first
-// version -- one CTA per image, each lane adding ~37 partials in a load -> add chain -- spent 22 us per call waiting for one L2 round
-// trip per addend), then a fixed-order reduction: lanes by shuffle, the eight warps through shared memory.  Deterministic.
+// of the image's tpi tiles.  grid (32 groups, N), 256 threads: every thread takes a few partials with INDEPENDENT loads (a
+// load -> add chain over all partials would wait for one L2 round trip per addend), then a fixed-order reduction: lanes by shuffle, the eight warps through shared memory.  Deterministic.
 constexpr int kFoldThreads = 256;
 __global__ void __launch_bounds__(kFoldThreads)
 gn_fold_kernel(const float* __restrict__ partials, float* __restrict__ sums, int mode, int G, int tpi, int octs, int oct0, int vpg) {

@@ -1,9 +1,9 @@
 // pdl.cuh -- programmatic dependent launch (griddepcontrol) helpers.
 //
-// A guided step is ~1.4 k back-to-back kernels on one stream; most of them run for 2 - 20 us, so the drain -> launch ->
+// A guided step is ~900 back-to-back kernels on one stream; most of them are short, so the drain -> launch ->
 // prologue bubble between two kernels is a first-order cost.  Kernels that use these helpers are launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization: the next kernel's CTAs become resident as soon as every CTA of the
-// current one has executed `pdl_launch_dependents()` (or exited), run their prologue (barrier init, TMEM alloc, descriptor
+// current one has executed `pdl_launch_dependents()` (or exited), run their prologue (barrier init, descriptor
 // prefetch, loads of step-invariant parameters) and block in `pdl_wait()` until the previous grid has completed and its
 // writes are visible.  Rules followed by every kernel in this library:
 //   * nothing that another kernel of the step writes is read, and no global memory is written, before pdl_wait();

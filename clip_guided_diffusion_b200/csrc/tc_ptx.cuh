@@ -1,4 +1,4 @@
-// tc_ptx.cuh -- inline-PTX wrappers for the Blackwell tensor-core path (mbarrier, TMA, tcgen05, clusters).
+// tc_ptx.cuh -- inline-PTX wrappers for the Hopper asynchronous data path (mbarrier, TMA, bulk copies, clusters / DSMEM).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -38,6 +38,12 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
   }
 }
+// Same bound without the printf: a call between wgmma issue and wait makes ptxas serialise every wgmma of the kernel (C7510).
+__device__ __forceinline__ void mbar_wait_trap(uint64_t* bar, uint32_t parity) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity))
+    if (++spins > (1u << 26)) __trap();
+}
 __device__ __forceinline__ void tma_load_4d(void* smem, const CUtensorMap* tm, uint64_t* bar, int c0, int c1, int c2, int c3) {
   asm volatile(
       "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
@@ -50,23 +56,6 @@ __device__ __forceinline__ void tma_load_2d(void* smem, const CUtensorMap* tm, u
       ::"r"(smem_u32(smem)), "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-// shared memory -> global tensor store (bulk async-group completion)
-__device__ __forceinline__ void tma_store_4d(const void* smem, const CUtensorMap* tm, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(tm), "r"(smem_u32(smem)), "r"(c0),
-               "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_group_read() {  // at most N groups still READING their shared-memory source
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-template <int N>
-__device__ __forceinline__ void bulk_wait_group() {
-  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
-}
-// generic-proxy shared-memory writes -> visible to the async proxy (TMA store source)
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 // 1-D bulk copy global -> shared (bytes % 16 == 0, both addresses 16-byte aligned), completion on an mbarrier
 __device__ __forceinline__ void bulk_load_1d(void* smem, const void* gmem, uint32_t bytes, uint64_t* bar) {
@@ -91,66 +80,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tm) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread = lane = accumulator row)
-__device__ __forceinline__ void tc_ld_32x32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tc_ld_32x16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tc_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major, 128B-swizzled operand tile: rows of 64 fp16 (128 B), 8-row swizzle atoms of 1024 B.
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);  // start address, bits [0,14)
-  d |= (uint64_t)0 << 16;                   // leading byte offset: unused for swizzled K-major (one atom along K)
-  d |= (uint64_t)(1024 >> 4) << 32;         // stride byte offset between 8-row atoms, bits [32,46)
-  d |= (uint64_t)1 << 46;                   // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                   // layout type SWIZZLE_128B
-  return d;
-}
-// kind::f16 instruction descriptor: fp16 x fp16 -> fp32, A and B K-major, M=128, N=BN
-__host__ __device__ constexpr uint32_t make_idesc_f16(int n) {
-  return (1u << 4)                    // D format fp32
-         | (0u << 7) | (0u << 10)     // A, B format fp16
-         | (0u << 15) | (0u << 16)    // A, B K-major
-         | ((uint32_t)(n >> 3) << 17) // N / 8
-         | ((uint32_t)(128 >> 4) << 24);  // M / 16
-}
-
-
-// ---- 2-CTA (cta_group::2) variants and cluster helpers
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // clears the CTA-pair peer bit of a shared::cluster address -> leader CTA's copy
-
+// ---- clusters and distributed shared memory
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -160,43 +90,16 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// arrive (count 1) on the barrier at the same smem offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 remAddr32;\n\t"
-      "mapa.shared::cluster.u32 remAddr32, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [remAddr32];\n\t}"
-      ::"r"(smem_u32(bar)), "r"(cta)
-      : "memory");
+// address of the same shared-memory location in CTA `cta` of the cluster
+__device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t cta) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(cta));
+  return r;
 }
-__device__ __forceinline__ void tma2_load_4d(void* smem, const CUtensorMap* tm, uint64_t* bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(smem)), "l"(tm), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma2_load_2d(void* smem, const CUtensorMap* tm, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem)), "l"(tm), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tc2_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-__device__ __forceinline__ void tc2_mma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// kind::f16 instruction descriptor with explicit M (128 for cta_group::1, 256 for cta_group::2)
-__host__ __device__ constexpr uint32_t make_idesc_f16_mn(int m, int n) {
-  return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+__device__ __forceinline__ float4 ld_cluster_f4(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
+  return v;
 }
 
 }  // namespace cgd

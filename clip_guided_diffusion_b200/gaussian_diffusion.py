@@ -112,7 +112,7 @@ class GaussianDiffusion:
     # ---- one step.  `model` is the engine's UNet handle (guidance.EngineModel)
     def p_mean_variance(self, model, x, t, clip_denoised=True, denoised_fn=None, model_kwargs=None):
         _require(not clip_denoised and denoised_fn is None,
-                 "the B200 step implements the reference's configuration (clip_denoised=False, no denoised_fn; cgd/cgd.py:253)")
+                 "the H100 step implements the reference's configuration (clip_denoised=False, no denoised_fn; cgd/cgd.py:253)")
         engine = _engine_of(model)
         return engine.unet_forward(self, x, _uniform_t(t), (model_kwargs or {}).get("y"))
 

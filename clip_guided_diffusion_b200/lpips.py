@@ -1,8 +1,8 @@
-"""LPIPS-VGG16 perceptual loss against an init image, as a B200 op plan: value and gradient with respect to x_in.
+"""LPIPS-VGG16 perceptual loss against an init image, as an H100 op plan: value and gradient with respect to x_in.
 
 Replaces [3P] ``lpips.LPIPS(net='vgg')`` as the reference uses it (cgd/cgd.py:147-148 lazy construction, 220-224
 ``lpips_vgg(x_in, init_tensor).sum() * init_scale`` inside the differentiated loss; SURVEY.md A.4, K21, section 8f row 3).  The
-13 conv3x3 layers run on the tcgen05 implicit-GEMM kernel (forward and dgrad), ReLU / 2x2 max-pool / the per-tap normalise-diff-
+13 conv3x3 layers run on the wgmma implicit-GEMM kernel (forward and dgrad), ReLU / 2x2 max-pool / the per-tap normalise-diff-
 lin-mean with its analytic gradient are the kernels of csrc/lpips.cu.  The init image's features are constant: they are
 computed once by the same forward ops and stored channel-normalised.  State dict keys follow the upstream layout
 (``net.sliceK.<vgg16.features index>.{weight,bias}``, ``linK.model.1.weight``).

@@ -79,28 +79,27 @@ def _round_up(a, b):
 
 
 def pick_bn(npad: int, m_tiles: int, kblocks: int = 1 << 30) -> int:
-    """Output-channel tile width.  The CTA-pair kernel runs ceil(tiles / 74) rounds of 74 clusters (148 SMs); wide tiles
-    amortise the A-operand traffic and the per-tile epilogue, narrow ones fill the machine: maximise utilisation x a
-    per-width efficiency prior (measured ordering on B200: 256 > 192 > 128 > 64).
+    """Output-channel tile width.  The conv kernel runs one 128-pixel x BN tile per CTA and one CTA per SM (its operand ring
+    takes most of the shared memory), so a layer takes ceil(tiles / N_SMS) rounds; wide tiles amortise the A-operand traffic
+    and the per-tile epilogue (a wgmma of N = 256 reads the same 64-row A slice as one of N = 64), narrow ones fill the
+    machine: maximise utilisation x a per-width efficiency prior (256 > 192 > 128 > 64).
     Short-K GEMMs (<= 16 K-blocks: 1x1 convs, the ViT's K = 768 Linears) that fit one round are latency-bound, not
-    tensor-bound: the narrowest tile that still fits one round wins and split-K (a second launch) never pays
-    (profiles/r01_conv_sweep_v1.txt: 768->768 at M = 800 runs 7.7 us with BN 64 against 17.2 us with BN 256 + split 2)."""
+    tensor-bound: the narrowest tile that still fits one round wins and split-K (a second launch) does not pay."""
     cands = [b for b in (256, 192, 128, 64, 32, 16) if npad % b == 0]
     big = [b for b in cands if b >= 64]
     if not big:
         return cands[0]
-    pair_tiles = (m_tiles + 1) // 2
     if kblocks <= 16:
-        one_round = [b for b in big if pair_tiles * (npad // b) <= 74]
+        one_round = [b for b in big if m_tiles * (npad // b) <= N_SMS]
         if one_round:
             return min(one_round)
     eff = {256: 1.0, 192: 0.95, 128: 0.85, 64: 0.6}
     best, best_score = big[0], -1.0
     for b in big:
-        tiles = pair_tiles * (npad // b)
-        rounds = -(-tiles // 74)
-        util = tiles / (rounds * 74.0)
-        if tiles < 74:  # split-K will add parallelism; do not punish wide tiles too hard
+        tiles = m_tiles * (npad // b)
+        rounds = -(-tiles // N_SMS)
+        util = tiles / (rounds * float(N_SMS))
+        if tiles < N_SMS:  # split-K will add parallelism; do not punish wide tiles too hard
             util = max(util, 0.6)
         score = util * eff[b]
         if score > best_score + 1e-9:
@@ -121,28 +120,27 @@ def conv_tile_count(NB, H, W):
 
 
 def pick_splits(m_tiles, n_tiles, kblocks, npad, ws_cap_bytes=16 << 20) -> int:
-    """split-K factor for layers whose output tiles cannot fill the 74 CTA pairs: aim at one full round, keep at least
+    """split-K factor for layers whose output tiles cannot fill the SMs: aim at one full round, keep at least
     6 K-blocks (of 64) per tile so the TMA/MMA pipeline amortises its fill, bound the fp32 partial workspace."""
-    tiles = ((m_tiles + 1) // 2) * n_tiles if m_tiles >= 2 else m_tiles * n_tiles
-    slots = 74 if m_tiles >= 2 else 148
-    if tiles * 2 > slots or kblocks <= 16:
+    tiles = m_tiles * n_tiles
+    if tiles * 2 > N_SMS or kblocks <= 16:
         return 1
-    s = min(kblocks // 6, slots // tiles, 32)
-    cap = ws_cap_bytes // (((m_tiles + 1) // 2 * 2) * 128 * npad * 4)
+    s = min(kblocks // 6, N_SMS // tiles, 32)
+    cap = ws_cap_bytes // (m_tiles * 128 * npad * 4)
     s = max(1, min(s, cap))
     per = -(-kblocks // s)
     return -(-kblocks // per)
 
 
-_T_KB = {64: 0.29, 128: 0.35, 192: 0.41, 256: 0.47}  # us per K-block per CTA of a pair (operand stream, profiles/r01_conv_sweep_v1.txt)
-
-
 _CLUSTER_CAP = {}
+# co-resident clusters of S CTAs of the conv kernel (one CTA per SM; the same for every tile width), cudaOccupancyMaxActiveClusters on
+# an H100 80GB HBM3 (132 SMs): the answers CPU plan builds use, so that they make the same choices as the device
+_H100_CLUSTER_CAP = {1: 132, 2: 66, 4: 30, 8: 15}
 
 
 def cluster_capacity(bn: int, S: int) -> int:
-    """co-resident clusters of 2*S CTAs for tile width bn: asked from the library on a CUDA box (cudaOccupancyMaxActiveClusters),
-    B200's answers (33 / 15 / 7 clusters of 4 / 8 / 16 CTAs) when there is no device (CPU plan builds: interpreter tests, op_report)"""
+    """co-resident clusters of S CTAs for tile width bn: asked from the library on a CUDA box (cudaOccupancyMaxActiveClusters),
+    the H100 answers when there is no device (CPU plan builds: interpreter tests, op_report)"""
     key = (bn, S)
     if key not in _CLUSTER_CAP:
         cap = -1
@@ -153,49 +151,37 @@ def cluster_capacity(bn: int, S: int) -> int:
                 cap = int(_lib.load().cgd_conv_cluster_capacity(bn, S))
         except Exception:
             cap = -1
-        _CLUSTER_CAP[key] = cap if cap >= 0 else {1: 74, 2: 33, 4: 15, 8: 7}[S]  # the B200 answers
+        _CLUSTER_CAP[key] = cap if cap >= 0 else _H100_CLUSTER_CAP[S]
     return _CLUSTER_CAP[key]
 
 
-# in-cluster split-K cost model, fitted to profiles/r01_cluster_sweep_v2.txt (in-graph times on B200): fixed us per (BN, S) -- launch,
-# two cluster barriers, the DSMEM exchange of a 128 x BN fp32 tile at ~20 B/clk per SM -- plus ~0.31 us per K-block per pair
-_CL_FIXED = {(64, 2): 7.2, (128, 2): 8.5, (192, 2): 9.6, (256, 2): 12.6, (64, 4): 7.0, (128, 4): 6.8, (192, 4): 8.5, (256, 4): 10.0,
-             (128, 8): 8.0, (256, 8): 9.6}
-
-
 def pick_cluster_split(m_tiles: int, npad: int, kblocks: int, cout: int):
-    """(BN, S, estimated us) for the in-cluster split-K kernel (csrc/conv_tc3.cu), or None.  One cluster of 2*S CTAs per output tile
-    of 256 pixels x BN channels; the whole launch must fit one wave of clusters (`cluster_capacity`: 33 / 15 / 7 clusters of
-    4 / 8 / 16 CTAs on B200); each pair gets >= 3 K-blocks and BN / S (the columns a pair reduces and stores) is a multiple of 16."""
+    """(BN, S, K-blocks per CTA) for the in-cluster split-K path of the conv kernel (csrc/conv_tc.cu, CONV i23), or None.  One
+    cluster of S CTAs per output tile of 128 pixels x BN channels; the whole launch must fit one wave of clusters
+    (`cluster_capacity`); each CTA gets >= 3 K-blocks and BN / S (the columns a CTA reduces and stores) is a multiple of 16.
+    The shortest K loop per CTA wins; ties go to the smaller cluster (less distributed-shared-memory traffic), then the wider tile."""
     if cout % 8:
         return None
-    pair_tiles = (m_tiles + 1) // 2
     best = None
     for bn in (256, 192, 128, 64):
         if npad % bn:
             continue
-        tiles = pair_tiles * (npad // bn)
+        tiles = m_tiles * (npad // bn)
         for S in (2, 4, 8):
             if bn % S or (bn // S) % 16 or tiles > cluster_capacity(bn, S):
                 continue
             kps = -(-kblocks // S)
             if kps < 3 or (S - 1) * kps >= kblocks:
                 continue
-            est = _CL_FIXED[(bn, S)] + kps * (0.31 + (0.06 if tiles > 8 else 0.0))
-            if best is None or est < best[2] - 1e-9:
-                best = (bn, S, est)
+            if best is None or kps < best[2]:
+                best = (bn, S, kps)
     return best
-
-
-def workspace_split_estimate(bn: int, splits: int, kblocks: int, rows: int, npad: int) -> float:
-    """us for the pair kernel writing `splits` fp32 partial tensors + the reduce launch (fit of the same sweep)"""
-    return 5.0 + -(-kblocks // splits) * _T_KB[bn] + 0.55 * splits * rows * npad * 4 / 1e6
 
 
 def gn_fused_cluster(N: int, HW: int, C: int, maxv: int) -> int:
     """Cluster size (CTAs along the pixel dimension) of the single-launch GroupNorm kernels (csrc/norm_fused.cu), or 0 when the
     two-pass kernels are the better choice.  512 threads, 16-byte vectors, at most `maxv` vectors per thread (16 forward,
-    8 backward), clusters of at most 4 CTAs.  Measured on B200 (profiles/r01_gn_microbench_v1.txt): a CTA reads only its groups'
+    8 backward), clusters of at most 4 CTAs.  A CTA reads only its groups'
     channels of every pixel (32-128 contiguous bytes), so beyond ~4 MB per image the partial-line traffic loses against the
     full-row two-pass kernels; below, the single launch wins by 2-4x."""
     if C % 256 != 0 or C > 4096 or HW * C > (2 << 20):
@@ -214,8 +200,8 @@ def gn_fused_cluster(N: int, HW: int, C: int, maxv: int) -> int:
     return cs
 
 
-N_SMS = 148  # B200
-GN_STREAM_CTAS = 148 * 8  # partial-sum slots of the streaming GroupNorm engine (csrc/norm_stream.cu: kGsMaxCtas)
+N_SMS = 132  # H100 SXM
+GN_STREAM_CTAS = 132 * 8  # partial-sum slots of the streaming GroupNorm engine (csrc/norm_stream.cu: kGsMaxCtas)
 
 
 def gn_partial_floats(N: int, gn_g: int) -> int:
@@ -244,14 +230,14 @@ class Plan:
         self._tape: list[Callable[[], None]] = []
         self._grads: dict = {}
         self.conv_impl = conv_impl
-        # long sequences (T % 256 == 0) as batched tcgen05 GEMMs + transposes + softmax kernels; superseded by the flash kernels of
+        # long sequences (T % 256 == 0) as batched tensor-core GEMMs + transposes + softmax kernels; superseded by the flash kernels of
         # csrc/attention_mma.cu (one launch forward, three backward, nothing T x T in HBM), kept for A/B measurements
         self.tc_attention = os.environ.get("CGD_TC_ATTENTION", "0") == "1"
-        # split-K reduced inside a thread-block cluster through DSMEM (csrc/conv_tc3.cu) instead of partials + a reduce launch
+        # split-K reduced inside a thread-block cluster through DSMEM (csrc/conv_tc.cu) instead of partials + a reduce launch
         self.cluster_splitk = os.environ.get("CGD_CONV_CLUSTER", "1") == "1"
-        # ... also for one-wave layers that did not need split-K to fill the machine but have long K loops: the 64 x 64 level's
-        # 512 -> 512 3x3 runs 27.0 instead of 36.3 us, 1024 -> 512 43.5 instead of 66.0 us; +1.4 % per step, same box
-        # (profiles/r02_call_w_cluster_wide_v1.log).  CGD_CLUSTER_WIDE=0 switches it off for A/B runs.
+        # ... also for one-wave layers that did not need split-K to fill the machine but have long K loops (the 64 x 64 level's
+        # 512 -> 512 and 1024 -> 512 3x3s): a wider tile split along K inside a cluster shortens the K loop per SM.
+        # CGD_CLUSTER_WIDE=0 switches it off for A/B runs.
         self.cluster_wide = os.environ.get("CGD_CLUSTER_WIDE", "1") == "1"
         # GroupNorm forward from statistics reduced in the producing conv's epilogue (CONV flags 2 + GN_APPLY_EPI): one streaming trip
         # instead of two.  Interpreter-verified, NOT yet run on the device: opt-in until it is (DESIGN.md "Next")
@@ -343,29 +329,27 @@ class Plan:
         splits = pick_splits(m_tiles, npad // bn, kblocks, npad)
         cluster = 0
         if splits > 1 and self.cluster_splitk and self.conv_impl in (0, 3) and b_ptr is None and not out_f32 and out_sc == 1:
+            # one launch and no fp32 partial tensor, unless the workspace split would give each CTA a shorter K loop
             pick = pick_cluster_split(m_tiles, npad, kblocks, Cout)
-            if pick is not None and pick[2] + 1.0 < workspace_split_estimate(bn, splits, kblocks, NB * H * W, npad):
+            if pick is not None and pick[2] <= -(-kblocks // splits):
                 bn, splits = pick[:2]
                 cluster = 1
         elif (splits == 1 and self.cluster_wide and self.cluster_splitk and self.conv_impl in (0, 3) and b_ptr is None and not out_f32 and out_sc == 1
+              and not res_gelu  # the QuickGELU' epilogue needs splits == 1 (conv_gelu_epilogue_ok)
               and m_tiles >= 2 and kblocks >= 32 and not (want_stats and self.gn_epi_stats)):
             # one wave of narrow tiles with a long K loop (the 64 x 64 level: 64 BN-128 tiles x 72 K-blocks = 33 us at 0.46 us per K-block):
             # wider tiles split along K inside a cluster can be shorter even though no split-K was "needed" to fill the machine
             pick = pick_cluster_split(m_tiles, npad, kblocks, Cout)
-            rounds = -(-(((m_tiles + 1) // 2) * (npad // bn)) // 74)
-            plain = 5.0 + rounds * kblocks * (_T_KB[bn] + 0.10)  # + 0.10: measured 0.46 us per K-block at BN 128 in one-wave layers
-            if pick is not None and pick[2] + 2.0 < plain:
+            rounds = -(-(m_tiles * (npad // bn)) // N_SMS)
+            if pick is not None and 2 * pick[2] <= rounds * kblocks:  # at least halves the K loop per SM
                 bn, splits = pick[:2]
                 cluster = 1
-        ws = skbar = None
-        if cluster:
-            pass
-        elif splits > 1:
-            ws = self.new(splits * ((m_tiles + 1) // 2 * 2) * 128 * npad, "f", "splitk_ws")
-            skbar = self.new(2 * ((m_tiles + 1) // 2 * 2) * (npad // bn), "u32", "splitk_bar")
+        ws = None
+        if splits > 1 and not cluster:
+            ws = self.new(splits * m_tiles * 128 * npad, "f", "splitk_ws")
         i = [NB, H, W, Cin, Cout, npad, taps, *x_strides, *out_strides, *(res_strides or (0, 0, 0)), bn, splits, self.conv_impl, out_sc,
              b_batch[0], b_batch[1], ldb, cluster]
-        # epilogue statistics for a following GroupNorm: pair kernel with the TMA-store epilogue, full 128-pixel tiles inside an image
+        # epilogue statistics for a following GroupNorm: tensor-core kernel without split-K, full 128-pixel tiles inside an image
         stats = None
         tw = 1
         while tw < W and tw < 128:
@@ -378,14 +362,14 @@ class Plan:
         if res_gelu:
             assert self.conv_gelu_epilogue_ok(NB, H, W, Cin, npad, Cout, taps), tag
         self.emit("CONV", flags=(1 if out_f32 else 0) | (2 if stats is not None else 0) | (4 if res_gelu else 0), i=i,
-                  p=[x_ptr, b_ptr if b_ptr is not None else self._bp(wbuf), self._bp(bias), res_ptr, out_ptr, self._bp(ws), self._bp(skbar)]
+                  p=[x_ptr, b_ptr if b_ptr is not None else self._bp(wbuf), self._bp(bias), res_ptr, out_ptr, self._bp(ws), None]
                   + ([self._bp(stats)] if stats is not None else []), tag=tag)
         return stats
 
     def conv_gelu_epilogue_ok(self, NB, H, W, Cin, npad, Cout, taps) -> bool:
-        """would this conv run on the pair kernel with the TMA-store epilogue (the one that implements CONV flags 4)?  Mirrors the
-        choices of `_emit_conv` / conv_tc_prepare: tcgen05 path, >= 2 pixel tiles, no split-K, BN >= 64, whole 64-channel chunks."""
-        if self.conv_impl not in (0, 3) or os.environ.get("CGD_CONV_EPI_TMA", "1") == "0" or os.environ.get("CGD_QGELU_EPI", "1") == "0":
+        """would this conv run with the epilogue that implements CONV flags 4?  Mirrors the choices of `_emit_conv` /
+        conv_tc_prepare: wgmma path, >= 2 pixel tiles, no split-K, BN >= 64, whole 64-channel chunks."""
+        if self.conv_impl not in (0, 3) or os.environ.get("CGD_QGELU_EPI", "1") == "0":
             return False
         m_tiles = conv_tile_count(NB, H, W)
         kblocks = taps * Cin // 64
@@ -651,7 +635,7 @@ class Plan:
         return out
 
     def _attention_tc(self, qkv: Act, heads: int, T: int, B: int, legacy_order: bool, name: str) -> Act:
-        """softmax(Q K^T / sqrt(d)) V for T % 256 == 0 as batched tcgen05 GEMMs (S and P materialised in fp16 like the
+        """softmax(Q K^T / sqrt(d)) V for T % 256 == 0 as batched tensor-core GEMMs (S and P materialised in fp16 like the
         reference's einsum / softmax(w.float()).type(dtype)), transposes so that every operand is K-major, row softmax."""
         C = qkv.C // 3
         d, ld = 64, qkv.ld

@@ -1,5 +1,5 @@
 """CLIP ``ModifiedResNet`` towers (RN50, RN101, RN50x4, RN50x16: the other `clip_model_name`s of cgd/clip_util.py:17) as an op list on the same kernels
-as the ViT tower: every layer is the tcgen05 conv (BatchNorm folded into weights and bias at build time -- the reference runs the
+as the ViT tower: every layer is the wgmma conv (BatchNorm folded into weights and bias at build time -- the reference runs the
 tower in eval mode, cgd/clip_util.py:64), ReLU, 2x2 average pooling, the small-T attention kernel for AttentionPool2d.
 
 Two layout tricks keep it on the existing kernels:

@@ -1,9 +1,9 @@
-"""ADM UNet (guided-diffusion ``UNetModel``) as a B200 op plan: forward and input-gradient backward.
+"""ADM UNet (guided-diffusion ``UNetModel``) as an H100 op plan: forward and input-gradient backward.
 
 Replaces [3P] ``guided_diffusion.unet.UNetModel.forward`` and the autograd walk of it that the reference triggers
 with ``th.autograd.grad(loss, x)`` (cgd/cgd.py:228); constructed from the same flags the reference merges at
 cgd/script_util.py:305-316 and from a state_dict in upstream key layout (SURVEY.md Appendix A.1, A.5), so real
-checkpoints load unchanged.  All convolutions (3x3, 1x1, qkv / proj) run on the tcgen05 implicit-GEMM kernel;
+checkpoints load unchanged.  All convolutions (3x3, 1x1, qkv / proj) run on the wgmma implicit-GEMM kernel;
 activations are pixel-major fp16 like the reference's ``convert_to_fp16`` trunk (cgd/script_util.py:322-323);
 GroupNorm statistics, the timestep-embedding MLP and all accumulation are fp32.
 """

@@ -1,9 +1,9 @@
-"""CLIP visual tower (``clip.model.VisionTransformer``) as a B200 op plan: encode_image forward and input gradient.
+"""CLIP visual tower (``clip.model.VisionTransformer``) as an H100 op plan: encode_image forward and input gradient.
 
 Replaces [3P] ``clip_model.encode_image`` (called at cgd/cgd.py:194) and its autograd backward (cgd/cgd.py:228).
 Weights come from a state_dict in upstream key layout (``visual.*``, SURVEY.md Appendix A.3, A.5).  The input is
 not an image tensor but the patch matrix that the cutout kernel writes directly in patch order, so the patch
-"convolution" is a plain GEMM.  Linear layers run on the tcgen05 GEMM kernel with fp16 operands / fp32
+"convolution" is a plain GEMM.  Linear layers run on the wgmma GEMM kernel with fp16 operands / fp32
 accumulation (the reference's CUDA path loads CLIP in fp16, cgd/clip_util.py:64-65); LayerNorm statistics,
 softmax and the final projection are fp32.
 """

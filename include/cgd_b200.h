@@ -1,5 +1,5 @@
 /*
- * cgd_b200.h -- C ABI of libcgd_b200.so: the B200 (sm_100a) kernels behind the reference's
+ * cgd_b200.h -- C ABI of libcgd_b200.so: the H100 (sm_90a) kernels behind the reference's
  * per-timestep CLIP-guided sampling step.
  *
  * The reference (afiaka87/clip-guided-diffusion) has no FFI of its own: its hot path is Python
@@ -33,7 +33,7 @@
 extern "C" {
 #endif
 
-#define CGD_ABI_VERSION 1
+#define CGD_ABI_VERSION 2  /* 2: CONV i23 clusters of `splits` CTAs (were 2 * splits), p6 unused, i18 = 3 no longer the narrow kernels */
 #define CGD_OP_NI 24
 #define CGD_OP_NF 8
 #define CGD_OP_NP 12
@@ -50,24 +50,24 @@ typedef struct CgdOp {
  * Slot tables: iN / fN / pN are CgdOp.i[N] / .f[N] / .p[N].  "h" = fp16, "f" = fp32.
  */
 enum {
-  /* Implicit-GEMM convolution / GEMM on tcgen05 tensor cores (TMA-fed, TMEM accumulators).
+  /* Implicit-GEMM convolution / GEMM on Hopper tensor cores (TMA-fed, wgmma, register accumulators).
    * Replaces [3P] UNet Conv2d 3x3 / 1x1, Conv1d k=1, and [3P] CLIP Linear / patch conv
    * (SURVEY K1-K3, K12, K13) in both directions (dgrad = same kernel, host-transformed weights).
    *   out[n,y,x,co] = sum_{tap,ci} A[n, y+dy(tap), x+dx(tap), ci] * Wp[co, tap*Cin+ci] (+bias[co]) (+res[n,y,x,co])
    *   p0 A(h)  p1 Wp(h, [Npad, taps*Cin] K-major)  p2 bias(f)|0  p3 res(h)|0  p4 out(h|f)  p5 splitK ws(f)|0
    *   i0 NB i1 H i2 W i3 Cin(%64==0) i4 Cout i5 Npad(%BN==0) i6 taps(1|9)
    *   i7..9 A strides (n,h,w)  i10..12 out strides  i13..15 res strides  i16 BN  i17 splits
-   *   i18 impl (0 = tcgen05, 1 = SIMT verification kernel)  i19 out channel stride (0/1 = contiguous; >1 only
+   *   i18 impl (0 = wgmma, with the mma.sync kernels for narrow / 8x8 layers; 1 = SIMT verification kernel; 2 = the wgmma tile kernel for
+   *   every layer, workspace split-K only; 3 = the wgmma tile kernel for every layer, with in-cluster split-K and the fused epilogues)  i19 out channel stride (0/1 = contiguous; >1 only
    *   with scalar stores, e.g. fp32 NCHW outputs of the UNet head / stem dgrad)
    *   i20, i21 batched-GEMM mode: element strides of the B operand per h / per n index (0, 0 = one shared weight matrix);
-   *   i22 row stride of B (0 = taps*Cin).  Batched mode needs W % 256 == 0 (attention: A = Q/P/dS..., B = K/V^T/...)
-   *   p6 split-K barrier words (u32 [2 * row tiles * channel tiles], zero-initialised)|0: when given and the launch fits one wave,
-   *   the kernel reduces its own split-K partials (no second launch)
-   *   i23 = 1: split-K inside a thread-block cluster of 2 * splits CTAs, reduced through distributed shared memory (one launch, no
+   *   i22 row stride of B (0 = taps*Cin).  Batched mode needs W > 64, one (h, n) per 128-pixel tile (attention: A = Q/P/dS..., B = K/V^T/...)
+   *   p6 unused (0)
+   *   i23 = 1: split-K inside a thread-block cluster of `splits` CTAs, reduced through distributed shared memory (one launch, no
    *   workspace; splits in 2..8, BN >= 64, BN / splits a multiple of 16, fp16 contiguous output, Cout % 8 == 0)
-   *   flags: 1 = out is fp32 ; 2 = epilogue statistics for CGD_OP_GN_APPLY_EPI into p7 (pair kernel with the TMA-store epilogue, full
+   *   flags: 1 = out is fp32 ; 2 = epilogue statistics for CGD_OP_GN_APPLY_EPI into p7 (wgmma kernel, no split-K, fp16 output, full
    *   128-pixel tiles inside one image) ; 4 = p3 is a QuickGELU pre-activation u and out = acc * QuickGELU'(u) instead of acc + res
-   *   (dgrad of the CLIP MLP's c_proj writing d c_fc directly; pair kernel with the TMA-store epilogue, no bias) */
+   *   (dgrad of the CLIP MLP's c_proj writing d c_fc directly; wgmma kernel, no split-K, Cout % 8 == 0, no bias) */
   CGD_OP_CONV = 1,
   /* GroupNorm(32) statistics: per (image, chunk, group) partial sum / sum of squares; the last block per image
    * folds the chunks (fixed order, fp64) into (mean, rstd).  [3P] GroupNorm32 (SURVEY K5).
@@ -269,7 +269,7 @@ enum {
 /* ------------------------------------------------------------------ entry points --------------- */
 int cgd_abi_version(void);
 const char* cgd_last_error(void);
-/* How many thread-block clusters of 2 * splits CTAs of the in-cluster split-K conv kernel (CONV i23 = 1, tile width bn in
+/* How many thread-block clusters of `splits` CTAs of the in-cluster split-K conv kernel (CONV i23 = 1, tile width bn in
  * {64, 128, 192, 256}) the current device holds at once (cudaOccupancyMaxActiveClusters); -1 without a device.  Plans use it to
  * keep such a layer within one wave of clusters. */
 int cgd_conv_cluster_capacity(int32_t bn, int32_t splits);

@@ -1,4 +1,4 @@
-"""In-cluster split-K (csrc/conv_tc3.cu) against the workspace split-K + reduce launch, per latency-bound layer shape: cluster
+"""In-cluster split-K (csrc/conv_tc.cu, CONV i23) against the workspace split-K + reduce launch, per latency-bound layer shape: cluster
 capacities of the device, then every (BN, S) timed inside a CUDA graph over rotating buffers.  python scripts/cluster_sweep.py"""
 import os, sys
 import torch as th
@@ -62,6 +62,6 @@ for shp in SHAPES:
                 continue
             P.pick_cluster_split = lambda m, n, k, c, bn=bn, S=S: (bn, S, 0.0)
             t, op = time_plan(*shp)
-            tiles = (mt + 1) // 2 * (P._npad(Cout) // bn)
-            print(f"    BN{bn:3d} cl{S}: {tiles:3d} clusters x {2 * S:2d} CTAs, {kps:3d} K-blocks/pair: {t:6.1f} us", flush=True)
+            tiles = mt * (P._npad(Cout) // bn)
+            print(f"    BN{bn:3d} cl{S}: {tiles:3d} clusters x {S:2d} CTAs, {kps:3d} K-blocks/CTA: {t:6.1f} us", flush=True)
     P.pick_cluster_split = ORIG_PICK

@@ -1,5 +1,4 @@
-"""Times single conv layers alone (rotating buffers > L2, CUDA events) for a list of shapes; CGD_CONV_DBG switches of the
-pair kernel (1 = no TMA, 2 = no MMA, 4 = no stores) isolate the pipeline legs.  Usage: python scripts/conv_microbench.py [bn]"""
+"""Times single conv layers alone (rotating buffers > L2, CUDA events) for a list of shapes.  Usage: python scripts/conv_microbench.py [bn]"""
 import os, sys
 import torch as th
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,7 +1,7 @@
 """Summarise an `ncu --set full ... --page raw --csv` export: one line per profiled launch with the numbers north_star asks for
 (tensor-pipe % of peak for the contractions, achieved DRAM GB/s and % for the streams) plus duration, grid, registers, occupancy,
 issue-slot use and L2 hit rate.
-    python scripts/ncu_summary.py profiles/r02_families_raw.csv > profiles/r02_families_summary.txt"""
+    python scripts/ncu_summary.py profiles/families_raw.csv > profiles/families_summary.txt"""
 import csv, re, sys
 rows = list(csv.reader(open(sys.argv[1])))
 hdr, units, data = rows[0], rows[1], rows[2:]

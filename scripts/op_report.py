@@ -1,7 +1,7 @@
 """Pair every op of the cfg2 step plan (or of the bench workload named by CGD_PROFILE_WORKLOAD; rebuilt on the CPU, shapes only) with its
 launch(es) in an ncu gpu__time_duration launch list of scripts/profile_step.py eager, and print time by op kind and shape.
 
-    python scripts/op_report.py profiles/r01_launches_cfg2_step_v5_warm.csv [kind-filter]
+    python scripts/op_report.py profiles/launches_cfg2_step.csv [kind-filter]
 """
 import collections, csv, os, re, sys
 import torch as th

@@ -1,7 +1,7 @@
 """One launch of every kernel family of the cfg2 guided step inside a cudaProfilerStart/Stop range, for
-    ncu --set full --clock-control none --import-source on --profile-from-start off -o gpurun_out/r02_families python scripts/profile_families.py
+    ncu --set full --clock-control none --import-source on --profile-from-start off -o profiles/families python scripts/profile_families.py
 The engine runs two eager steps first (every buffer holds real data), then the chosen ops are launched one by one: for each op code
-the instance(s) with the most work, for CONV one per kernel variant / regime (pair kernel 3x3 dominant, with residual, 1x1, in-cluster
+the instance(s) with the most work, for CONV one per kernel variant / regime (wgmma tile kernel 3x3 dominant, with residual, 1x1, in-cluster
 split-K, workspace split-K + reduce, fp32 NCHW head / stem dgrad, ViT GEMMs)."""
 import os
 import sys

@@ -25,7 +25,7 @@ def test_header_symbols_exported(lib):
     assert declared == set(_lib.EXPORTS), declared ^ set(_lib.EXPORTS)
     for name in declared:
         assert hasattr(lib, name), name
-    assert lib.cgd_abi_version() == 1
+    assert lib.cgd_abi_version() == 2
 
 
 def test_op_tables_match_header():
@@ -75,7 +75,7 @@ def test_header_is_plain_c(tmp_path):
                         "-l:libcgd_b200.so", f"-Wl,-rpath,{libdir}"], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
     out = subprocess.run([str(exe)], capture_output=True, text=True)
-    assert out.returncode == 0 and out.stdout.split() == ["1", str(8 + 24 * 8 + 8 * 4 + 12 * 8)], out.stdout + out.stderr
+    assert out.returncode == 0 and out.stdout.split() == ["2", str(8 + 24 * 8 + 8 * 4 + 12 * 8)], out.stdout + out.stderr
 
 
 def test_product_path_never_imports_the_oracle():

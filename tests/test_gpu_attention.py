@@ -56,6 +56,7 @@ def _ref(qkv, heads, legacy):
     return o.reshape(qkv.shape[0], qkv.shape[1], -1)
 
 
+# id "tcgen05_gemms" kept stable across the port: the batched-GEMM formulation, now on the wgmma conv kernel
 @pytest.mark.parametrize("tc", [False, True], ids=["flash", "tcgen05_gemms"])
 @pytest.mark.parametrize("case", CASES, ids=[_case_id(c) for c in CASES])
 def test_attention_fwd_bwd(case, tc):
@@ -66,7 +67,7 @@ def test_attention_fwd_bwd(case, tc):
     C = heads * d
     th.manual_seed(0)
     plan = Plan()
-    plan.tc_attention = tc  # False: flash kernels (attention_small.cu / attention_mma.cu); True: batched tcgen05 GEMMs
+    plan.tc_attention = tc  # False: flash kernels (attention_small.cu / attention_mma.cu); True: batched wgmma GEMMs
     qkv = Act(plan.new(B * T * 3 * C, "h", "qkv"), 0, 1, 1, B * T, 3 * C, 3 * C)
     out = plan.attention(qkv, heads, T, B, legacy_order=legacy, name="attn")
     do = Act(plan.new(B * T * C, "h", "do"), 0, 1, 1, B * T, C, C)

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 implicit-GEMM conv / GEMM kernel (and its SIMT verification twin) against a plain PyTorch fp32
+"""GPU: the wgmma implicit-GEMM conv / GEMM kernel (and its SIMT verification twin) against a plain PyTorch fp32
 reference of the same op, across tile geometries, paddings, split-K, epilogues and output layouts."""
 import pytest
 import torch as th
@@ -30,7 +30,7 @@ CASES = [
     ("conv1x1_16x16_k3072", 1, 16, 16, 3072, 1024, 1, True, False),
     ("linear_k2304_m800", 1, 1, 800, 2304, 768, 1, False, True),              # BN 192, S = 4, ragged last pixel tile
     # the dominant layer of the benchmarked configuration: 31 % of the 256x256 UNet's FLOPs (M = 65536, N = 256, K = 2304), the
-    # shape bench.py's `roofline` line times -- 256 tiles on 74 CTA pairs (3.46 waves), with and without the ResBlock residual
+    # shape bench.py's `roofline` line times -- 512 tiles of 128 pixels, with and without the ResBlock residual
     ("conv3x3_256x256_c256_dominant", 1, 256, 256, 256, 256, 9, True, False),
     ("conv3x3_256x256_c256_dominant_res", 1, 256, 256, 256, 256, 9, True, True),
     ("conv3x3_256x256_c512_to_256", 1, 256, 256, 512, 256, 9, True, False),      # output blocks at 256x256: K = 4608
@@ -41,7 +41,7 @@ CASES = [
     ("conv1x1_8x8_qkv", 1, 8, 8, 1024, 3072, 1, True, False),
     ("conv1x1_8x8_proj_res_b2", 2, 8, 8, 1024, 1024, 1, True, True),
     ("conv1x1_8x8_k3072", 1, 8, 8, 3072, 1024, 1, True, False),
-    ("conv3x3_8x8_c2048_to_1024", 1, 8, 8, 2048, 1024, 9, True, False),   # K too large for the slab: stays on the tcgen05 split-K path
+    ("conv3x3_8x8_c2048_to_1024", 1, 8, 8, 2048, 1024, 9, True, False),   # K too large for the slab: stays on the wgmma split-K path
     # widths of the 128x128 checkpoint (channel_mult 1, 1, 2, 3, 4: a 768-wide 16x16 level, 1280 / 1792-wide concatenations)
     ("conv3x3_16x16_c768_res", 1, 16, 16, 768, 768, 9, True, True),
     ("conv3x3_16x16_c1792_to_768", 1, 16, 16, 1792, 768, 9, True, False),
@@ -64,11 +64,13 @@ def _ref_conv(x, w, b, res, taps):
     return y + res.float() if res is not None else y
 
 
+# ids (kept stable across the port): tc1 = impl 2, the wgmma tile kernel for every layer with workspace split-K; tc2pair = impl 3, the
+# same kernel for every layer with in-cluster split-K; tc2pair_ws_splitk = impl 3 with the in-cluster reduction switched off
 @pytest.mark.parametrize("impl", [0, 1, 2, 3, 13], ids=["auto", "simt", "tc1", "tc2pair", "tc2pair_ws_splitk"])
 @pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
 def test_conv_fwd_and_dgrad(case, impl):
     name, NB, H, W, Cin, Cout, taps, has_b, has_r = case
-    cluster = impl != 13  # 13: the pair kernel with the workspace split-K + reduce launch instead of the in-cluster reduction
+    cluster = impl != 13  # 13: impl 3 with the workspace split-K + reduce launch instead of the in-cluster reduction
     impl = 3 if impl == 13 else impl
     if impl == 1 and NB * H * W * Cout * taps * Cin > 3e10:
         pytest.skip("SIMT twin only on small cases")
@@ -145,18 +147,6 @@ def test_conv_special_layouts(impl):
     assert float(gott[:, 0].abs().max()) == 0.0  # cls rows untouched
 
 
-def test_co_resident_pair_kernel_instantiation():
-    """CGD_CONV_CO=1: latency-bound launches (one wave of tiles or a short K loop) take the pair kernel's two-CTAs-per-SM
-    instantiation with a short operand ring (csrc/conv_tc2.cu, CO).  The switch is read once per process: every conv case is re-run
-    in a child process with it on."""
-    import os, subprocess, sys
-    env = dict(os.environ, CGD_CONV_CO="1")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, "-m", "pytest", "tests/test_gpu_conv.py", "-q", "-x", "-m", "gpu", "-k", "(auto or tc2pair or special) and not co_resident",
-                        "-p", "no:cacheprovider"], cwd=root, env=env, capture_output=True, text=True, timeout=1200)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]
-
-
 @pytest.mark.parametrize("rows", [800, 200])
 def test_quick_gelu_backward_fused_into_dgrad_epilogue(rows):
     """CLIP MLP: a = QuickGELU(u), y = c_proj(a).  The dgrad of c_proj multiplies its accumulator by QuickGELU'(u) in the epilogue
@@ -215,7 +205,7 @@ def test_narrow_conv_halo_kernel(shape):
 
 def test_small_image_weight_streaming_kernel():
     """CGD_CONV_SMALL=1: 8 x 8 images take conv_small_kernel (csrc/conv_narrow.cu: a CTA per 8 output channels streaming its whole
-    weight slab, TMA box per activation slice, mma.sync) instead of split-K tcgen05 tiles.  Opt-in (measured break-even); the switch
+    weight slab, TMA box per activation slice, mma.sync) instead of split-K wgmma tiles.  Opt-in (measured break-even); the switch
     is read once per process, so the 8 x 8 cases are re-run in a child process with it on."""
     import os, subprocess, sys
     env = dict(os.environ, CGD_CONV_SMALL="1")

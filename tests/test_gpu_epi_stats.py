@@ -7,7 +7,7 @@ import pytest
 import torch as th
 import torch.nn.functional as F
 
-pytestmark = pytest.mark.gpu  # device-validated in round 2 (gpurun call A: passed on a B200), no longer opt-in
+pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("shape", [(1, 128, 128, 256, 256, True), (2, 64, 64, 128, 512, False), (1, 256, 256, 256, 256, True)],

@@ -1,7 +1,7 @@
 """GPU, BASELINE.json full sizes.
 cfg1 (64x64 checkpoint architecture, respace 25, batch 1, cutn 4, ViT-B/32, use_magnitude auto-on): teacher-forced step vs the
 fp32 oracle on the host CPU.  cfg2 (256x256, cutn 16): too slow for the CPU oracle inside a test, so it is checked through
-size-independent properties: tcgen05 path == SIMT verification twin on the full UNet, graph replay == eager (bitwise),
+size-independent properties: wgmma path == SIMT verification twin on the full UNet, graph replay == eager (bitwise),
 linearity of the input-gradient backward in its seed."""
 import pytest
 import torch as th

@@ -1,4 +1,4 @@
-"""GPU: the LPIPS-VGG16 init loss (clip_guided_diffusion_b200/lpips.py + csrc/lpips.cu + the tcgen05 conv kernel): every op against
+"""GPU: the LPIPS-VGG16 init loss (clip_guided_diffusion_b200/lpips.py + csrc/lpips.cu + the wgmma conv kernel): every op against
 the PyTorch interpreter on identical inputs, loss value and x_in-gradient against the fp32 oracle restatement of
 ``lpips.LPIPS(net='vgg')`` ([3P], cgd/cgd.py:147-148, 220-224; SURVEY.md A.4)."""
 import pytest

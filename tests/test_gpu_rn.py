@@ -5,7 +5,7 @@ import os
 import pytest
 import torch as th
 
-pytestmark = pytest.mark.gpu  # device-validated in round 2 (gpurun call A: passed on a B200), no longer opt-in
+pytestmark = pytest.mark.gpu
 
 
 def test_rn_tower_matches_oracle_on_device():

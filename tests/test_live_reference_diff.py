@@ -1,138 +1,100 @@
-"""CPU, build container only (skipped where /root/reference does not exist, e.g. on the GPU box): differential tests against the LIVE
-reference -- its importable modules (`cgd.modules`, `cgd.losses`) and the function bodies of `cgd/script_util.py` cut out with `ast`
-(the module itself does not import).  The committed goldens under tests/golden/ pin a handful of seeds; this widens the same
-comparisons to many random inputs while the reference is at hand."""
-import ast
+"""CPU: differential tests against the reference on many random inputs -- its modules (`cgd.modules`, `cgd.losses`), the function
+bodies of `cgd/script_util.py` and the `cond_fn` closure of `cgd/cgd.py`.  The inputs are generated here from fixed seeds;
+`tests/golden/live_reference_golden.json.gz` / `.npz` hold what the reference returned for them (tests/golden/make_golden_live_reference.py
+runs it).  Tensor outputs are stored as a fixed, seeded sample of their elements (plus the absolute maximum), to keep the files small."""
+import gzip
+import hashlib
+import json
 import os
 import random
-import re
-import sys
 
+import numpy as np
 import pytest
 import torch as th
 
-REF = "/root/reference"
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "cgd")), reason="the reference tree is only present in the build container")
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+N_SAMPLE = 256
 
 
-def _ref_script_util():
-    ns = {"os": os, "re": re}
-    src = open(os.path.join(REF, "cgd", "script_util.py")).read()
-    for node in ast.parse(src).body:
-        if isinstance(node, ast.FunctionDef) and node.name in ("parse_prompt", "alphanumeric_filter", "clean_and_combine_prompts"):
-            exec(compile(ast.Module([node], []), "cgd/script_util.py", "exec"), ns)
-    return ns
+def _golden():
+    with gzip.open(os.path.join(GOLDEN, "live_reference_golden.json.gz"), "rt", encoding="utf-8") as f:
+        js = json.load(f)
+    return js, dict(np.load(os.path.join(GOLDEN, "live_reference_golden.npz")))
 
 
-def _ref_modules():
-    if REF not in sys.path:
-        sys.path.append(REF)  # appended: nothing of this repository may be shadowed
-    from cgd import losses, modules
-    return losses, modules
+def sample_index(numel: int, key: str) -> th.Tensor:
+    """fixed element sample of a tensor output: all of it when small, else N_SAMPLE indices drawn from a generator seeded by `key`"""
+    if numel <= N_SAMPLE:
+        return th.arange(numel)
+    seed = int(hashlib.sha256(key.encode()).hexdigest()[:8], 16)
+    return th.randperm(numel, generator=th.Generator().manual_seed(seed))[:N_SAMPLE].sort().values
 
 
-def test_prompt_helpers_on_random_strings():
-    from clip_guided_diffusion_b200 import cgd
-    ref = _ref_script_util()
+def summarize(t: th.Tensor, key: str) -> np.ndarray:
+    """[absmax, sampled elements...] of a tensor output, float64"""
+    flat = t.detach().double().flatten()
+    return np.concatenate([[float(flat.abs().max()) if flat.numel() else 0.0], flat[sample_index(flat.numel(), key)].numpy()])
+
+
+def rng_digest() -> str:
+    return hashlib.sha256(th.get_rng_state().numpy().tobytes()).hexdigest()
+
+
+def _close(got: th.Tensor, want: np.ndarray, key: str, rel: float):
+    g = summarize(got, key)
+    assert g.shape == want.shape, key
+    assert abs(g[0] - want[0]) <= rel * want[0] + 1e-12, (key, g[0], want[0])
+    assert np.abs(g[1:] - want[1:]).max(initial=0.0) <= rel * want[0] + 1e-12, key
+
+
+# ---------------------------------------------------------------- inputs (shared with the golden script)
+ALPHABET = "abc XYZ019_-.,:;!?/\\'\"()[]{}<>@#$%^&*+=~`|\t\néü中\U0001f600"
+N_PROMPTS = 600
+
+
+def prompt_cases():
+    """(texts, b) for the filter / combine helpers, then prompts for parse_prompt"""
     rng = random.Random(7)
-    alphabet = "abc XYZ019_-.,:;!?/\\'\"()[]{}<>@#$%^&*+=~`|\t\néü中\U0001f600"
-    for _ in range(2000):
-        texts = ["".join(rng.choice(alphabet) for _ in range(rng.randint(0, n))) for n in (40, 300)]
-        b = rng.randint(0, 99)
-        assert cgd.alphanumeric_filter(texts[0]) == ref["alphanumeric_filter"](texts[0])
-        assert cgd.clean_and_combine_prompts("base", texts, b) == ref["clean_and_combine_prompts"]("base", texts, b)
+    combine = []
+    for _ in range(N_PROMPTS):
+        texts = ["".join(rng.choice(ALPHABET) for _ in range(rng.randint(0, n))) for n in (40, 300)]
+        combine.append((texts, rng.randint(0, 99)))
+    prompts = []
     for _ in range(2000):
         body = "".join(rng.choice("ab :/.-") for _ in range(rng.randint(0, 12)))
-        prompt = rng.choice(["", "http://", "https://"]) + body + rng.choice(["", ":1", ":-0.5", ":2e-1", ":3", ":", ":x"])
-        try:
-            want = ref["parse_prompt"](prompt)
-        except ValueError:  # "text:" / "text:x": float('') raises in the reference, so it must here
-            with pytest.raises(ValueError):
-                cgd.parse_prompt(prompt)
-            continue
-        assert cgd.parse_prompt(prompt) == want, prompt
+        prompts.append(rng.choice(["", "http://", "https://"]) + body + rng.choice(["", ":1", ":-0.5", ":2e-1", ":3", ":", ":x"]))
+    return combine, prompts
 
 
-def test_cutout_windows_follow_the_reference_generator_for_random_geometries():
-    """same CPU-generator consumption and the same windows as cgd/modules.py:26-48 for random image sizes, cut sizes, counts, powers --
-    fresh draws, cached draws and the `num_cutouts_override` prefix rule; product class and oracle class"""
-    from clip_guided_diffusion_b200 import guidance as pg
-    from oracle import guidance as og
-    _, modules = _ref_modules()
+def cutout_cases():
     rng = random.Random(11)
+    out = []
     for trial in range(300):
         cs = rng.choice([32, 224, 288, 336, 384])
         side_x, side_y = rng.choice([64, 128, 256, 320, 512]), rng.choice([64, 128, 256, 320, 512])
         cutn, power = rng.randint(1, 40), rng.choice([1.0, 0.5, 2.0, 0.25])
-        ref = modules.MakeCutouts(cs, cutn, cutout_size_power=power)
-        for mk in (pg.MakeCutouts(cs, cutn, cutout_size_power=power), og.MakeCutouts(cs, cutn, power)):
-            th.manual_seed(trial)
-            want = ref._generate_coords(side_x, side_y, cutn)
-            state = th.get_rng_state()
-            th.manual_seed(trial)
-            assert mk._generate_coords(side_x, side_y, cutn) == want
-            assert th.equal(th.get_rng_state(), state), "different consumption of the default generator"
-            th.manual_seed(trial + 1)
-            ref.cache_coordinates(side_x, side_y)
-            th.manual_seed(trial + 1)
-            mk.cache_coordinates(side_x, side_y)
-            assert mk.cached_coords == ref.cached_coords
-    # the product's coords_for() mirrors forward()'s choice between the cache and fresh draws (cgd/modules.py:50-58)
-    mk, ref = pg.MakeCutouts(224, 16), modules.MakeCutouts(224, 16)
-    th.manual_seed(3)
-    ref.cache_coordinates(256, 256)
-    th.manual_seed(3)
-    mk.cache_coordinates(256, 256)
-    assert mk.coords_for(256, 256, use_cache=True, num_cutouts_override=4) == ref.cached_coords[:4]
-    th.manual_seed(4)
-    want = ref._generate_coords(256, 256, 8)
-    th.manual_seed(4)
-    assert mk.coords_for(256, 256, use_cache=False, num_cutouts_override=8) == want
+        out.append((trial, cs, side_x, side_y, cutn, power))
+    return out
 
 
-def test_oracle_cutouts_and_losses_equal_the_reference_modules_on_random_inputs():
-    from oracle import guidance as og
-    losses, modules = _ref_modules()
+def loss_cases():
+    """per trial: (B, H, W, x, seed, e, t, cutout weight or None) -- drawn in the order the comparisons consume them"""
     g = th.Generator().manual_seed(5)
+    out = []
     for trial in range(12):
         B, H, W = [1, 2, 3][trial % 3], [48, 64, 40][trial % 3], [48, 40, 64][(trial // 3) % 3]
-        x = (th.randn(B, 3, H, W, generator=g) * 1.5).requires_grad_()
+        x = th.randn(B, 3, H, W, generator=g) * 1.5
         seed = th.randn(B, generator=g)
-        for ours, theirs in ((og.range_loss, losses.range_loss), (og.tv_loss, losses.tv_loss)):
-            a, b = ours(x), theirs(x)
-            ga, gb = th.autograd.grad((a * seed).sum(), x)[0], th.autograd.grad((b * seed).sum(), x)[0]
-            assert th.equal(a, b) and th.equal(ga, gb)
-        e, t = th.randn(1, 5, B, 16, generator=g).requires_grad_(), th.randn(1, 1, 16, generator=g)
-        a, b = og.spherical_dist_loss(e, t), losses.spherical_dist_loss(e, t)
-        assert th.equal(a, b) and th.equal(th.autograd.grad(a.sum(), e)[0], th.autograd.grad(b.sum(), e)[0])
-        if H >= W:  # wide images make the reference's swapped axes produce empty crops (RuntimeError in adaptive_avg_pool2d)
-            cutn = 4
-            th.manual_seed(trial)
-            want = modules.MakeCutouts(32, cutn)(x)
-            th.manual_seed(trial)
-            got = og.MakeCutouts(32, cutn)(x)
-            assert th.equal(got, want)
-            w = th.randn(want.shape, generator=g)
-            assert th.equal(th.autograd.grad((got * w).sum(), x)[0], th.autograd.grad((want * w).sum(), x)[0])
+        e, t = th.randn(1, 5, B, 16, generator=g), th.randn(1, 1, 16, generator=g)
+        w = th.randn(B * 4, 3, 32, 32, generator=g) if H >= W else None  # wide images: empty crops in the reference (no comparison)
+        out.append((trial, B, H, W, x, seed, e, t, w))
+    return out
 
 
-def test_oracle_cond_fn_equals_the_live_reference_closure_on_random_configurations():
-    """the committed cond_fn goldens widened: 40 random (batch, prompts, image size, cutouts, power, chain length, timestep, scales,
-    saturation, magnitude) configurations, reference closure (cgd/cgd.py:151-239, compiled from its source) vs `OracleCondFn`"""
-    import importlib.util
-    import types
+def cond_cases():
     from oracle import diffusion as od
-    from oracle import guidance as og
-    _ref_modules()
-    spec = importlib.util.spec_from_file_location("make_golden_cond_fn", os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "make_golden_cond_fn.py"))
-    mg = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mg)
-    while REF in sys.path[:1]:  # the script puts the reference first on sys.path for its own run: move it back behind this repository
-        sys.path.remove(REF)
-        sys.path.append(REF)
-    from cgd.modules import MakeCutouts as RefMakeCutouts
-    code = mg.reference_cond_fn_code()
     rng = random.Random(3)
+    out = []
     for trial in range(40):
         B = rng.choice([1, 1, 2, 3])
         P = 1 if B > 1 else rng.choice([1, 2, 4])  # quirk B1: the broadcast is only defined for B == 1 or P == 1
@@ -147,15 +109,86 @@ def test_oracle_cond_fn_equals_the_live_reference_closure_on_random_configuratio
         w = th.randn(P, generator=g).abs() + 0.1
         w = w / w.sum().abs()
         diff = od.create_gaussian_diffusion(1000, "linear", str(T))
-        ns = mg.make_closure(code, diffusion=types.SimpleNamespace(num_timesteps=T, sqrt_one_minus_alphas_cumprod=diff.sqrt_one_minus_alphas_cumprod),
-                             current_timestep=t, num_cutouts=cutn, make_cutouts=RefMakeCutouts(32, cutn, cutout_size_power=power), clip_model=mg.StubClip(32, 16),
-                             target_embeds=target, weights=w, sat_scale=sat, use_saturation=sat != 0, use_magnitude=mag, **scales)
-        th.manual_seed(trial)
-        xr = x.clone().requires_grad_()
-        want = ns["cond_fn"](xr, th.full((B,), t), {"pred_xstart": mg.stub_pred_xstart(xr)}).detach()
-        cond = og.OracleCondFn(diff, mg.StubClip(32, 16), target, w, cut_size=32, num_cutouts=cutn, cutout_power=power, sat_scale=sat, use_magnitude=mag, **scales)
+        out.append(dict(trial=trial, B=B, P=P, H=H, W=W, cutn=cutn, power=power, T=T, t=t, sat=sat, mag=mag, scales=scales, x=x, target=target,
+                        w=w, diff=diff))
+    return out
+
+
+# ---------------------------------------------------------------- tests
+def test_prompt_helpers_on_random_strings():
+    from clip_guided_diffusion_b200 import cgd
+    js, _ = _golden()
+    combine, prompts = prompt_cases()
+    want = js["prompts"]
+    for (texts, b), (filt, comb) in zip(combine, want["combine"], strict=True):
+        assert cgd.alphanumeric_filter(texts[0]) == filt
+        assert cgd.clean_and_combine_prompts("base", texts, b) == comb
+    for prompt, ref in zip(prompts, want["parse"], strict=True):
+        if ref is None:  # "text:" / "text:x": float('') raises in the reference, so it must here
+            with pytest.raises(ValueError):
+                cgd.parse_prompt(prompt)
+            continue
+        assert list(cgd.parse_prompt(prompt)) == ref, prompt
+
+
+def test_cutout_windows_follow_the_reference_generator_for_random_geometries():
+    """same CPU-generator consumption and the same windows as cgd/modules.py:26-48 for random image sizes, cut sizes, counts, powers --
+    fresh draws, cached draws and the `num_cutouts_override` prefix rule; product class and oracle class"""
+    from clip_guided_diffusion_b200 import guidance as pg
+    from oracle import guidance as og
+    js, _ = _golden()
+    for (trial, cs, side_x, side_y, cutn, power), ref in zip(cutout_cases(), js["cutouts"], strict=True):
+        want = [tuple(c) for c in ref["coords"]]
+        cached = [tuple(c) for c in ref["cached"]]
+        for mk in (pg.MakeCutouts(cs, cutn, cutout_size_power=power), og.MakeCutouts(cs, cutn, power)):
+            th.manual_seed(trial)
+            assert [tuple(c) for c in mk._generate_coords(side_x, side_y, cutn)] == want
+            assert rng_digest() == ref["rng"], "different consumption of the default generator"
+            th.manual_seed(trial + 1)
+            mk.cache_coordinates(side_x, side_y)
+            assert [tuple(c) for c in mk.cached_coords] == cached
+    # the product's coords_for() mirrors forward()'s choice between the cache and fresh draws (cgd/modules.py:50-58)
+    mk = pg.MakeCutouts(224, 16)
+    th.manual_seed(3)
+    mk.cache_coordinates(256, 256)
+    assert [tuple(c) for c in mk.coords_for(256, 256, use_cache=True, num_cutouts_override=4)] == [tuple(c) for c in js["coords_for"]["cached"][:4]]
+    th.manual_seed(4)
+    assert [tuple(c) for c in mk.coords_for(256, 256, use_cache=False, num_cutouts_override=8)] == [tuple(c) for c in js["coords_for"]["fresh"]]
+
+
+def test_oracle_cutouts_and_losses_equal_the_reference_modules_on_random_inputs():
+    from oracle import guidance as og
+    _, gold = _golden()
+    for trial, B, H, W, x, seed, e, t, w in loss_cases():
+        x = x.clone().requires_grad_()
+        for name, fn in (("range", og.range_loss), ("tv", og.tv_loss)):
+            a = fn(x)
+            ga = th.autograd.grad((a * seed).sum(), x)[0]
+            _close(a, gold[f"loss{trial}_{name}"], f"loss{trial}_{name}", 1e-6)
+            _close(ga, gold[f"loss{trial}_{name}_grad"], f"loss{trial}_{name}_grad", 1e-6)
+        e = e.clone().requires_grad_()
+        a = og.spherical_dist_loss(e, t)
+        _close(a, gold[f"loss{trial}_sph"], f"loss{trial}_sph", 1e-6)
+        _close(th.autograd.grad(a.sum(), e)[0], gold[f"loss{trial}_sph_grad"], f"loss{trial}_sph_grad", 1e-6)
+        if w is not None:
+            th.manual_seed(trial)
+            got = og.MakeCutouts(32, 4)(x)
+            _close(got, gold[f"loss{trial}_cut"], f"loss{trial}_cut", 1e-6)
+            _close(th.autograd.grad((got * w).sum(), x)[0], gold[f"loss{trial}_cut_grad"], f"loss{trial}_cut_grad", 1e-6)
+
+
+def test_oracle_cond_fn_equals_the_live_reference_closure_on_random_configurations():
+    """the committed cond_fn goldens widened: 40 random (batch, prompts, image size, cutouts, power, chain length, timestep, scales,
+    saturation, magnitude) configurations, reference closure (cgd/cgd.py:151-239, compiled from its source) vs `OracleCondFn`"""
+    from oracle import guidance as og
+    from tests.test_cond_fn_reference import StubClip, stub_pred_xstart
+    _, gold = _golden()
+    for c in cond_cases():
+        trial, B, t = c["trial"], c["B"], c["t"]
+        cond = og.OracleCondFn(c["diff"], StubClip(32, 16), c["target"], c["w"], cut_size=32, num_cutouts=c["cutn"], cutout_power=c["power"],
+                               sat_scale=c["sat"], use_magnitude=c["mag"], **c["scales"])
         cond.current_timestep = t
         th.manual_seed(trial)
-        xr = x.clone().requires_grad_()
-        got = cond(xr, th.full((B,), t), {"pred_xstart": mg.stub_pred_xstart(xr)})
-        assert float((got - want).abs().max()) <= 1e-5 * float(want.abs().max()) + 1e-12, (trial, B, P, H, W, cutn, T, t, sat, mag)
+        xr = c["x"].clone().requires_grad_()
+        got = cond(xr, th.full((B,), t), {"pred_xstart": stub_pred_xstart(xr)})
+        _close(got, gold[f"cond{trial}"], f"cond{trial}", 1e-5)

@@ -126,8 +126,8 @@ def test_param_inventories_match_oracle():
 
 
 def test_cluster_split_picks_are_eligible():
-    """plan.pick_cluster_split only returns configurations the C side accepts (csrc/conv_tc3.cu: conv_cluster_split_ok) and that fit
-    one wave of clusters; every K split is non-empty."""
+    """plan.pick_cluster_split only returns configurations the C side accepts (csrc/conv_tc.cu: the CONV i23 check of conv_tc_prepare)
+    and that fit one wave of clusters (one cluster of S CTAs per 128-pixel x BN tile); every K split is non-empty."""
     from clip_guided_diffusion_b200 import plan as P
     seen = 0
     for (NB, H, W) in [(1, 8, 8), (2, 8, 8), (1, 16, 16), (1, 32, 32), (1, 64, 64), (1, 1, 800), (1, 1, 3152), (4, 16, 16),
@@ -141,14 +141,14 @@ def test_cluster_split_picks_are_eligible():
                     pick = P.pick_cluster_split(m_tiles, npad, kb, cout)
                     if pick is None:
                         continue
-                    bn, S, est = pick
+                    bn, S, kb_per_cta = pick
                     seen += 1
                     assert bn in (64, 128, 192, 256) and npad % bn == 0 and 2 <= S <= 8
                     assert bn % S == 0 and (bn // S) % 16 == 0 and cout % 8 == 0
                     kps = -(-kb // S)
                     assert (S - 1) * kps < kb and kps >= 3            # no empty split, a pipeline worth filling
-                    assert (m_tiles + 1) // 2 * (npad // bn) <= P.cluster_capacity(bn, S)
-                    assert est > 0
+                    assert m_tiles * (npad // bn) <= P.cluster_capacity(bn, S)
+                    assert kb_per_cta == kps
     assert seen > 50
     assert P.pick_cluster_split(2, 1024, 144, 1023) is None  # Cout % 8 != 0: the vector epilogue cannot store it
 
