@@ -51,9 +51,6 @@ static int dispatch(const CgdOp& op, const ConvTcLaunch* conv, cudaStream_t st) 
     case CGD_OP_COPY: return launch_copy(op, st);
     case CGD_OP_ATTN_FWD: return launch_attn_fwd(op, st);
     case CGD_OP_ATTN_BWD: return launch_attn_bwd(op, st);
-    case CGD_OP_TRANSPOSE: return launch_transpose(op, st);
-    case CGD_OP_SOFTMAX_FWD: return launch_softmax_fwd(op, st);
-    case CGD_OP_SOFTMAX_BWD: return launch_softmax_bwd(op, st);
     case CGD_OP_GN_FWD_FUSED: return launch_gn_fwd_fused(op, st);
     case CGD_OP_GN_BWD_FUSED: return launch_gn_bwd_fused(op, st);
     case CGD_OP_GN_FWD_GRID: return launch_gn_fwd_grid(op, st);
@@ -72,7 +69,6 @@ static int dispatch(const CgdOp& op, const ConvTcLaunch* conv, cudaStream_t st) 
     case CGD_OP_MAG_CLAMP: return launch_mag_clamp(op, st);
     case CGD_OP_ATTNPOOL_EMBED_FWD: return launch_attnpool_embed_fwd(op, st);
     case CGD_OP_ATTNPOOL_EMBED_BWD: return launch_attnpool_embed_bwd(op, st);
-    case CGD_OP_GN_APPLY_EPI: return launch_gn_apply_epi(op, st);
     case CGD_OP_LINEAR_SMALL: return launch_linear_small(op, st);
     case CGD_OP_TIMESTEP_EMB: return launch_timestep_emb(op, st);
     case CGD_OP_LABEL_ADD: return launch_label_add(op, st);
@@ -100,12 +96,12 @@ static int op_launches(const CgdOp& op, const ConvTcLaunch* conv) {
     case CGD_OP_CONV: return conv_tc_num_launches(*conv);
     case CGD_OP_ATTN_BWD: return attn_bwd_num_launches(op);
     case CGD_OP_FINAL_GRAD: return ((op.flags & 1) && !(op.flags & 4)) ? 2 : 1;
-    case CGD_OP_GN_FWD_GRID:
-    case CGD_OP_GN_BWD_GRID: return gn_grid_num_launches(op);
-    case CGD_OP_GN_APPLY_EPI: return gn_apply_epi_num_launches(op);
     default: return 1;
   }
 }
+
+// codes of removed ops (include/cgd_b200.h): rejected when the plan is built rather than when it runs
+static bool op_retired(int32_t code) { return code == 30 || code == 31 || code == 32 || code == 49; }
 
 static int plan_create(const CgdOp* ops, int32_t n_ops, Plan** out) {
   CGD_CHECK_ARG(ops != nullptr && n_ops > 0 && out != nullptr, "plan_create: bad arguments");
@@ -114,7 +110,7 @@ static int plan_create(const CgdOp* ops, int32_t n_ops, Plan** out) {
   pl->ops.assign(ops, ops + n_ops);
   pl->conv_index.assign(n_ops, -1);
   for (int i = 0; i < n_ops; ++i) {
-    if (ops[i].code <= 0 || ops[i].code >= CGD_OP__COUNT) {
+    if (ops[i].code <= 0 || ops[i].code >= CGD_OP__COUNT || op_retired(ops[i].code)) {
       set_error("plan_create: op %d has unknown code %d", i, ops[i].code);
       delete pl;
       return -1;
@@ -139,7 +135,7 @@ static int plan_create(const CgdOp* ops, int32_t n_ops, Plan** out) {
   if (!(getenv("CGD_CONV_PREFETCH") && getenv("CGD_CONV_PREFETCH")[0] == '0')) {
     for (size_t k = 0; k + 1 < pl->convs.size(); ++k) {
       const ConvTcLaunch& nx = pl->convs[k + 1];
-      if (nx.impl == 1 || nx.p.b_batched) continue;
+      if (nx.impl == 1) continue;
       pl->convs[k].p.pf_ptr = nx.Wp;
       pl->convs[k].p.pf_bytes = (int64_t)nx.p.Npad * nx.ldb * 2;
     }

@@ -3,8 +3,7 @@
 //
 // Replaces [3P] CLIP nn.MultiheadAttention's core for ViT-B/32 (50 tokens) and [3P] guided-diffusion QKVAttention(Legacy) at the
 // 8x8 UNet level (64 tokens) (SURVEY.md K4, K14).  Why a separate kernel: these problems are one 64x64 tile per head -- the
-// wgmma conv kernel wants 128-row tiles (conv_tc.cu) and the fp32 CUDA-core flash kernels of attention.cu need three launches
-// for the backward of such tiles.  Here the
+// flash kernels of attention_mma.cu need two launches for the backward.  Here the
 // whole backward -- S, P, dP, dS, dQ, dK, dV -- is one launch; P and dS go through shared memory once (fp16, like the
 // reference's fp16 attention weights) to feed the transposed products.
 #include <cuda_fp16.h>

@@ -141,12 +141,6 @@ __device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return ma
 __device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 #ifdef CGD_SIGMOID_EX2RCP
-// silu on a pair: t * 1 / (1 + 2^(-log2e * t))
-__device__ __forceinline__ float2 silu2(float2 t) {
-  const float2 u = mul2(t, make_float2(-1.4426950408889634f, -1.4426950408889634f));
-  const float2 d = add2(make_float2(ex2_ftz(u.x), ex2_ftz(u.y)), make_float2(1.f, 1.f));
-  return mul2(t, make_float2(rcp_ftz(d.x), rcp_ftz(d.y)));
-}
 // d silu / dt on a pair: s * (1 + t * (1 - s))
 __device__ __forceinline__ float2 silu_grad2(float2 t) {
   const float2 u = mul2(t, make_float2(-1.4426950408889634f, -1.4426950408889634f));
@@ -157,11 +151,6 @@ __device__ __forceinline__ float2 silu_grad2(float2 t) {
   return mul2(s, w);
 }
 #else
-// silu on a pair: with h = t / 2, t * sigmoid(t) = h * tanh(h) + h  (one MUFU and two packed ops per pair element)
-__device__ __forceinline__ float2 silu2(float2 t) {
-  const float2 h = mul2(t, make_float2(0.5f, 0.5f));
-  return fma2(h, make_float2(tanh_approx(h.x), tanh_approx(h.y)), h);
-}
 // d silu / dt on a pair: s * (1 + t * (1 - s)), s = 1/2 + 1/2 tanh(t / 2)
 __device__ __forceinline__ float2 silu_grad2(float2 t) {
   const float2 half2v = make_float2(0.5f, 0.5f), one = make_float2(1.f, 1.f);

@@ -45,8 +45,7 @@ struct TcCfg {
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStageLd = BN + 4;  // fp32 staging row stride (floats): 16-byte aligned rows, rows shifted across banks
   static constexpr int kStagingBytes = BM * kStageLd * 4;
-  static constexpr int kAuxBytes = 256 /*barriers*/ + BN * 4 /*epilogue statistics exchange: 4 row quarters x BN/8 octets x 2*/;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + kAuxBytes;
+  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(kStagingBytes <= kStages * kStageBytes, "the fp32 staging tile reuses the operand ring");
   static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 };
@@ -62,7 +61,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   float* staging = reinterpret_cast<float*>(smem);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
   uint64_t* empty_bar = full_bar + Cfg::kStages;
-  float* stat_red = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes + 256);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -105,7 +103,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           dx = tap % 3 - 1;
         }
         tma_load_4d(smem_a + stage * Cfg::kABytes, &tmA, &full_bar[stage], cb * BK, w0 + dx, h0 + dy, n0);
-        tma_load_4d(smem_b + stage * Cfg::kBBytes, &tmB, &full_bar[stage], kb * BK, ncol0, p.b_batched ? h0 : 0, p.b_batched ? n0 : 0);
+        tma_load_4d(smem_b + stage * Cfg::kBBytes, &tmB, &full_bar[stage], kb * BK, ncol0, 0, 0);
         if (++stage == Cfg::kStages) {
           stage = 0;
           phase ^= 1;
@@ -199,7 +197,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         continue;
       }
       const int col = ncol0 + c;
-      float st_s = 0.f, st_q = 0.f;  // flags 2: this row's sum / sum of squares of the octet's fp16 outputs
       if (row_ok && col < p.Cout) {
         if (col + 8 <= p.Cout && vec_ok) {
           if (p.bias) {
@@ -222,17 +219,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               for (int e = 0; e < 8; ++e) a[e] += rr[e];
             }
           }
-          const half8 hv = pack8(a);
-          st8(reinterpret_cast<__half*>(p.out) + o_off + col, hv);
-          if (p.epi_stats) {  // statistics of the ROUNDED values: what the GroupNorm after this conv reads
-            float f[8];
-            unpack8(hv, f);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              st_s += f[e];
-              st_q = fmaf(f[e], f[e], st_q);
-            }
-          }
+          st8(reinterpret_cast<__half*>(p.out) + o_off + col, pack8(a));
         } else {
           for (int e = 0; e < 8 && col + e < p.Cout; ++e) {
             float x = a[e];
@@ -242,23 +229,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             else reinterpret_cast<__half*>(p.out)[o_off + (col + e) * p.out_sc] = __float2half_rn(x);
           }
         }
-      }
-      if (p.epi_stats) {  // 32 rows -> one value per octet and row quarter (warp-uniform branch: full tiles, host)
-        st_s = warp_sum(st_s);
-        st_q = warp_sum(st_q);
-        if (lane == 0) {
-          stat_red[(quad * (BN / 8) + c / 8) * 2] = st_s;
-          stat_red[(quad * (BN / 8) + c / 8) * 2 + 1] = st_q;
-        }
-      }
-    }
-    if (p.epi_stats) {
-      named_bar_sync(1, kConsumers);
-      if ((int)threadIdx.x < BN / 4) {  // thread (octet o = t / 2, kind = t % 2): fixed-order sum over the four row quarters
-        const int o = threadIdx.x >> 1, kind = threadIdx.x & 1, stride = (BN / 8) * 2;
-        const float* src = stat_red + o * 2 + kind;
-        const float v = (src[0] + src[stride]) + (src[2 * stride] + src[3 * stride]);
-        p.epi_stats[((size_t)mt * (p.Npad / 8) + (size_t)(ncol0 / 8 + o)) * 2 + kind] = v;
       }
     }
   }
@@ -329,7 +299,7 @@ __global__ void conv_splitk_reduce_kernel(const ConvTcParams p, int m_tiles) {
 // cross-check the wgmma path layer by layer and so a tensor-core regression cannot block bring-up of the
 // rest of the step; never selected by the shipped plans (impl = 0).
 __global__ void conv_simt_kernel(const __half* __restrict__ A, const __half* __restrict__ Wp, const ConvTcParams p,
-                                 int64_t a_sn, int64_t a_sh, int64_t a_sw, int64_t ldb, int64_t b_sh, int64_t b_sn) {
+                                 int64_t a_sn, int64_t a_sh, int64_t a_sw, int64_t ldb) {
   pdl_wait();
   pdl_launch_dependents();
   const int64_t total = (int64_t)p.NB * p.H * p.W * p.Cout;
@@ -346,7 +316,7 @@ __global__ void conv_simt_kernel(const __half* __restrict__ A, const __half* __r
       const int yy = h + dy, xx = w + dx;
       if (yy < 0 || yy >= p.H || xx < 0 || xx >= p.W) continue;
       const __half2* a = reinterpret_cast<const __half2*>(A + n * a_sn + yy * a_sh + xx * a_sw);
-      const __half2* wr = reinterpret_cast<const __half2*>(Wp + (int64_t)co * ldb + (int64_t)tap * p.Cin + (int64_t)h * b_sh + (int64_t)n * b_sn);
+      const __half2* wr = reinterpret_cast<const __half2*>(Wp + (int64_t)co * ldb + (int64_t)tap * p.Cin);
       for (int c = 0; c < p.Cin / 2; ++c) {
         const float2 av = __half22float2(a[c]), wv = __half22float2(wr[c]);
         acc = fmaf(av.x, wv.x, acc);
@@ -397,6 +367,7 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
   ConvTcParams& p = L.p;
   const int64_t NB = op.i[0], H = op.i[1], W = op.i[2], Cin = op.i[3], Cout = op.i[4], Npad = op.i[5], taps = op.i[6];
   const int64_t BN = op.i[16], splits = op.i[17] > 0 ? op.i[17] : 1;
+  CGD_CHECK_ARG(op.i[20] == 0 && op.i[21] == 0 && op.i[22] == 0 && (op.flags & 2) == 0, "conv: i20..i22 and flags 2 are reserved and must be 0");
   CGD_CHECK_ARG(NB > 0 && H > 0 && W > 0, "conv: bad image dims %lld %lld %lld", (long long)NB, (long long)H, (long long)W);
   // tile counts, pixel indices and the TMA box arithmetic below are 32-bit: reject sizes whose pixel count does not fit instead of
   // overflowing (a 2^31-row "image" used to spin in pick_tile's power-of-two search)
@@ -436,13 +407,12 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
   const bool want_cluster = op.i[23] == 1 && op.i[18] != 1;  // plan flag; the SIMT twin ignores it
   if (p.splits > 1 && !want_cluster) CGD_CHECK_ARG(p.ws != nullptr, "conv: split-K needs a workspace");
   p.cluster = 0;
-  p.epi_stats = nullptr;  // set below when CONV flags 2 asks for epilogue statistics
   L.BN = (int)BN;
   L.impl = (int)op.i[18];
   L.A = reinterpret_cast<const __half*>(op.p[0]);
   L.Wp = reinterpret_cast<const __half*>(op.p[1]);
   L.a_sn = op.i[7]; L.a_sh = op.i[8]; L.a_sw = op.i[9];
-  L.ldb = op.i[22] > 0 ? op.i[22] : taps * Cin; L.b_sh = op.i[20]; L.b_sn = op.i[21];
+  L.ldb = taps * Cin;
   L.m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
   p.ws_rows = L.m_tiles * BM;
   L.n_tiles = (int)(Npad / BN);
@@ -461,16 +431,12 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
                   (int)r, (long long)Cin, (long long)W, (long long)H, (long long)NB, (long long)strides[0], (long long)strides[1],
                   (long long)strides[2], p.TW, p.TH, p.TN);
   }
-  const int64_t ldb = op.i[22] > 0 ? op.i[22] : taps * Cin;
-  p.b_batched = (op.i[20] != 0 || op.i[21] != 0) ? 1 : 0;
-  CGD_CHECK_ARG(ldb % 8 == 0 && op.i[20] % 8 == 0 && op.i[21] % 8 == 0, "conv: B strides must be multiples of 8 elements");
-  if (p.b_batched) CGD_CHECK_ARG(p.TH == 1 && p.TN == 1, "conv: batched-B GEMMs need W > 64 (one (h, n) per 128-pixel tile)");
   {
-    // 4-D map (K, rows, h, n) so batched GEMMs pick their B matrix by the tile's (h, n); plain weights use (0, 0)
-    const cuuint64_t K = (cuuint64_t)(taps * Cin);
-    const cuuint64_t row_bytes = (cuuint64_t)ldb * 2 * (cuuint64_t)Npad;
-    cuuint64_t dims4[4] = {K, (cuuint64_t)Npad, (cuuint64_t)(p.b_batched ? H : 1), (cuuint64_t)(p.b_batched ? NB : 1)};
-    cuuint64_t strides4[3] = {(cuuint64_t)ldb * 2, p.b_batched ? (cuuint64_t)op.i[20] * 2 : row_bytes, p.b_batched ? (cuuint64_t)op.i[21] * 2 : row_bytes};
+    // [Npad, K] weights as a 4-D map with unit outer dimensions (the kernel's loads are 4-D)
+    const cuuint64_t K = (cuuint64_t)L.ldb;
+    const cuuint64_t row_bytes = K * 2 * (cuuint64_t)Npad;
+    cuuint64_t dims4[4] = {K, (cuuint64_t)Npad, 1, 1};
+    cuuint64_t strides4[3] = {K * 2, row_bytes, row_bytes};
     cuuint32_t box4[4] = {64, (cuuint32_t)BN, 1, 1};
     cuuint32_t estr4[4] = {1, 1, 1, 1};
     CUresult r = enc(&L.tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, op.p[1], dims4, strides4, box4, estr4, CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -478,7 +444,7 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
     CGD_CHECK_ARG(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled(W) failed with %d", (int)r);
   }
   if (want_cluster) {
-    CGD_CHECK_ARG(L.impl != 1 && !p.out_f32 && p.out_sc == 1 && !p.b_batched && p.Cout % 8 == 0 && L.BN >= 64 && p.splits >= 2 && p.splits <= 8 &&
+    CGD_CHECK_ARG(L.impl != 1 && !p.out_f32 && p.out_sc == 1 && p.Cout % 8 == 0 && L.BN >= 64 && p.splits >= 2 && p.splits <= 8 &&
                       L.BN % p.splits == 0 && (L.BN / p.splits) % 16 == 0,
                   "conv: layer flagged for cluster split-K is not eligible (BN=%d splits=%d Cout=%d f32=%d)", L.BN, p.splits, p.Cout, p.out_f32);
     p.cluster = 1;
@@ -491,16 +457,6 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
                   "operand and no bias (BN=%d splits=%d Cout=%lld)", (int)BN, p.splits, (long long)Cout);
     p.res_mode = 1;
   }
-  // flags 2: the epilogue also reduces its output tile to per-octet sums for the GroupNorm that follows (GN_APPLY_EPI): needs the
-  // tensor-core kernel without split-K, fp16 contiguous output, and tiles that are full and are 128 consecutive pixels of one image
-  p.epi_stats = nullptr;
-  if (op.flags & 2) {
-    CGD_CHECK_ARG(L.impl != 1 && p.splits == 1 && !p.out_f32 && p.out_sc == 1 && op.p[7] != nullptr && W % p.TW == 0 && H % p.TH == 0 && p.TN == 1 &&
-                      (p.TW == W || p.TH == 1),
-                  "conv: epilogue statistics need the tensor-core kernel without split-K, fp16 output and full 128-pixel tiles inside one image (W=%lld H=%lld tile %dx%dx%d)",
-                  (long long)W, (long long)H, p.TW, p.TH, p.TN);
-    p.epi_stats = reinterpret_cast<float*>(op.p[7]);
-  }
   // <= 8 output channels, fp32 output, 3x3 (UNet head, stem dgrad): halo-tile mma.sync kernel (conv_narrow.cu); CGD_CONV_NARROW=0 keeps
   // the wgmma N = 16 tile for A/B runs
   {
@@ -510,28 +466,6 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
       narrow_on = (e && e[0] == '0') ? 0 : 1;
     }
     L.narrow = (narrow_on && conv_narrow_eligible(L)) ? 1 : 0;
-  }
-  // 8 x 8 images (deepest UNet level): one launch, a CTA per 8 output channels streaming its whole weight slab (conv_narrow.cu,
-  // conv_small_kernel) instead of split-K tiles + a reduce launch.  Opt-in (CGD_CONV_SMALL=1): not measured against the wgmma
-  // split-K path on the H100.
-  {
-    static int small_on = -1;
-    if (small_on < 0) {
-      const char* e = getenv("CGD_CONV_SMALL");
-      small_on = (e && e[0] == '1') ? 1 : 0;
-    }
-    L.small = (small_on && !L.narrow && conv_small_eligible(L)) ? 1 : 0;
-    L.tmS = L.tmA;
-    if (L.small) {  // one TMA box per 64-channel slice: the 8 x 8 image with its zero border (out-of-image coordinates are zero-filled)
-      const cuuint32_t e = taps == 9 ? 10 : 8;
-      cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)NB};
-      cuuint64_t strides[3] = {(cuuint64_t)op.i[9] * 2, (cuuint64_t)op.i[8] * 2, (cuuint64_t)op.i[7] * 2};
-      cuuint32_t box[4] = {64, e, e, 1};
-      cuuint32_t estr[4] = {1, 1, 1, 1};
-      CUresult r = enc(&L.tmS, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, op.p[0], dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      CGD_CHECK_ARG(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled(8x8 image box) failed with %d", (int)r);
-    }
   }
   return 0;
 }
@@ -611,7 +545,7 @@ int conv_cluster_capacity(int BN, int S) {
   }
 }
 
-// impl: 0 = auto, 1 = SIMT verification twin, 2 / 3 = the wgmma tile kernel for every layer (no narrow / 8 x 8 special kernels;
+// impl: 0 = auto, 1 = SIMT verification twin, 2 / 3 = the wgmma tile kernel for every layer (no narrow special kernel;
 // the plan uses in-cluster split-K and the fused epilogues with 0 and 3 only)
 int conv_tc_launch(const ConvTcLaunch& L, cudaStream_t st) {
   if (L.impl == 1) {
@@ -619,11 +553,10 @@ int conv_tc_launch(const ConvTcLaunch& L, cudaStream_t st) {
     const int blocks = (int)std::min<int64_t>(ceil_div(total, 256), (int64_t)device_sm_count() * 16);
     ConvTcParams p = L.p;
     p.splits = 1;
-    CGD_CUDA(launch_pdl(conv_simt_kernel, dim3(blocks), dim3(256), 0, st, L.A, L.Wp, p, L.a_sn, L.a_sh, L.a_sw, L.ldb, L.b_sh, L.b_sn));
+    CGD_CUDA(launch_pdl(conv_simt_kernel, dim3(blocks), dim3(256), 0, st, L.A, L.Wp, p, L.a_sn, L.a_sh, L.a_sw, L.ldb));
     return 0;
   }
   if (L.narrow) return conv_narrow_launch(L, st);
-  if (L.small) return conv_small_launch(L, st);
   int rc = 0;
   switch (L.BN) {
     case 16: rc = launch_tc<16>(L, st); break;
@@ -644,7 +577,7 @@ int conv_tc_launch(const ConvTcLaunch& L, cudaStream_t st) {
 }
 
 int conv_tc_num_launches(const ConvTcLaunch& L) {
-  return (L.impl != 1 && !L.small && !L.narrow && L.p.splits > 1 && !L.p.cluster) ? 2 : 1;
+  return (L.impl != 1 && !L.narrow && L.p.splits > 1 && !L.p.cluster) ? 2 : 1;
 }
 
 }  // namespace cgd

@@ -14,7 +14,6 @@ struct ConvTcParams {
   int tiles_w, tiles_h, tiles_n;
   int kblocks, splits, kb_per_split; // K loop = taps * Cin/64 blocks, optionally split over gridDim.z
   int out_f32;
-  int b_batched;                     // B operand indexed by the tile's (h, n) (batched GEMM: attention)
   int ws_rows;                       // rows per split in the split-K workspace (= m_tiles * 128)
   int cluster;                       // split-K inside a cluster of `splits` CTAs along z, reduced through distributed shared memory
   const void* pf_ptr;                // next conv's packed weights: prefetched into L2 by the idle lanes of the TMA warp (0 = none)
@@ -28,20 +27,17 @@ struct ConvTcParams {
   float* ws;                         // split-K partials [splits][m_tiles*128][Npad]
   int res_mode;                      // 0 = out = acc (+bias) + res ; 1 = out = acc * QuickGELU'(res) (CONV flags 4: the dgrad of the ViT's
                                      // c_proj writes d(c_fc output) directly, `res` = the saved pre-activation)
-  float* epi_stats;                  // flags 2: per (128-pixel tile, 8-channel octet) sum / sum of squares of the fp16 OUTPUT, [m_tiles][Npad/8][2]
 };
 
 struct ConvTcLaunch {
-  CUtensorMap tmA, tmB;              // A: 4-D pixel box; B: 4-D (K, rows, h, n) map, [BN x 64] weight slice per load
-  CUtensorMap tmS;                   // 8 x 8 images (conv_small_kernel): the whole image + zero border as one [64 ch x 10 x 10 x 1] box (3x3) / [64 x 8 x 8 x 1] (1x1)
+  CUtensorMap tmA, tmB;              // A: 4-D pixel box; B: [Npad, K] weights (4-D map, unit outer dims), [BN x 64] weight slice per load
   ConvTcParams p;
   int BN, impl, m_tiles, n_tiles;
-  int small;                         // 8 x 8 images: the weight-streaming mma.sync kernel of conv_narrow.cu (8 output channels per CTA, no split-K)
   int narrow;                        // <= 8 output channels, fp32 out, 3x3: the halo-tile mma.sync kernel of conv_narrow.cu instead of a wgmma tile
   const __half* A;
   const __half* Wp;
   int64_t a_sn, a_sh, a_sw;
-  int64_t ldb, b_sh, b_sn;
+  int64_t ldb;
 };
 
 int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L);
@@ -49,8 +45,6 @@ int conv_tc_launch(const ConvTcLaunch& L, cudaStream_t st);
 int conv_tc_num_launches(const ConvTcLaunch& L);
 bool conv_narrow_eligible(const ConvTcLaunch& L);              // conv_narrow.cu
 int conv_narrow_launch(const ConvTcLaunch& L, cudaStream_t st);
-bool conv_small_eligible(const ConvTcLaunch& L);
-int conv_small_launch(const ConvTcLaunch& L, cudaStream_t st);
 int conv_cluster_capacity(int BN, int S);
 
 }  // namespace cgd

@@ -13,9 +13,9 @@
 // the ring, whose loads are largely L2 hits (the tensors are 8 - 67 MB, the L2 is 50 MB) and start while the barrier is still
 // being crossed.  HBM traffic: x once + y once (forward), dy + x once + dx (backward).
 //
+// The large backward launches of widths C % 256 == 0 run on the direct-load kernel of norm_grid2.cu instead (gn_bwd_direct below).
+//
 // Replaces [3P] guided-diffusion GroupNorm32 + SiLU + scale-shift and their autograd (SURVEY.md K5, K6).
-#include <cstdlib>
-
 #include "common.cuh"
 #include "ops.cuh"
 #include "pdl.cuh"
@@ -429,37 +429,12 @@ static int gng_check(const char* what, int64_t N, int64_t HW, int64_t C, int64_t
                 what, (long long)N, (long long)Gn, kGngCtasPerSm, sms);
   return 0;
 }
-// norm_grid2.cu: the direct-load engine (C % 256 == 0)
+// norm_grid2.cu: the direct-load backward (C % 256 == 0)
 bool gn_grid2_supports(int64_t C);
-int launch_gn_fwd_grid2(const CgdOp& op, cudaStream_t st);
 int launch_gn_bwd_grid2(const CgdOp& op, cudaStream_t st);
-// norm_stream.cu: the streaming engine (three short launches: partial statistics, fold, apply; C % 256 == 0)
-bool gn_stream_supports(int64_t C);
-int gn_stream_partial_floats(int64_t N, int64_t HW, int64_t C);
-int launch_gn_fwd_stream(const CgdOp& op, cudaStream_t st);
-int launch_gn_bwd_stream(const CgdOp& op, cudaStream_t st);
-// Engines behind GN_FWD_GRID / GN_BWD_GRID: persistent ring, persistent direct (used for the large backward launches, where it keeps
-// more bytes in flight), and the streaming engine (three launches, norm_stream.cu), opt-in; none of the three has been compared on
-// the H100
-// (needs C % 256 == 0 and room in the op's partials buffer: i6 forward / i7 backward = capacity in floats).
-// CGD_GN_GRID_ENGINE = ring | direct | stream forces one engine for A/B runs.
-enum { kEngRing = 0, kEngDirect = 1, kEngStream = 2 };
-static int gng_engine(bool backward, int64_t N, int64_t HW, int64_t C, int64_t cap_floats) {
-  static int forced = -1;
-  if (forced < 0) {
-    const char* e = getenv("CGD_GN_GRID_ENGINE");
-    forced = !e ? 0 : (e[0] == 'r' ? 1 : (e[0] == 'd' ? 2 : (e[0] == 's' ? 3 : 0)));
-  }
-  const bool stream_ok = gn_stream_supports(C) && cap_floats >= gn_stream_partial_floats(N, HW, C);
-  if (forced == 3) return stream_ok ? kEngStream : (gn_grid2_supports(C) ? kEngDirect : kEngRing);
-  if (forced == 1 || !gn_grid2_supports(C)) return kEngRing;
-  if (forced == 2) return kEngDirect;
-  return (backward && HW * C >= (int64_t(1) << 23)) ? kEngDirect : kEngRing;  // streaming engine: opt-in (see norm_stream.cu header)
-}
-int gn_grid_num_launches(const CgdOp& op) {  // for cgd_plan_num_launches
-  const bool bwd = op.code == CGD_OP_GN_BWD_GRID;
-  return gng_engine(bwd, op.i[0], op.i[1], op.i[2], bwd ? op.i[7] : op.i[6]) == kEngStream ? 3 : 1;
-}
+// Every forward runs on the ring kernels of this file.  A backward of a large activation (HW * C >= 2^23) whose width the direct-load
+// kernel takes runs on that kernel, which keeps more bytes in flight; smaller ones stay on the ring.
+static bool gn_bwd_direct(int64_t HW, int64_t C) { return gn_grid2_supports(C) && HW * C >= (int64_t(1) << 23); }
 
 template <typename K>
 static int gng_prepare(K kernel) {
@@ -474,9 +449,6 @@ int launch_gn_fwd_grid(const CgdOp& op, cudaStream_t st) {
   const int64_t N = op.i[0], HW = op.i[1], C = op.i[2], ldx = op.i[3], ldy = op.i[4], Gn = op.i[5];
   if (int rc = gng_check("gn_fwd_grid", N, HW, C, Gn)) return rc;
   CGD_CHECK_ARG(ldx % 8 == 0 && ldy % 8 == 0 && op.p[0] && op.p[1] && op.p[2] && op.p[4] && op.p[5] && op.p[6] && op.p[7], "gn_fwd_grid: bad args");
-  const int eng = gng_engine(false, N, HW, C, op.i[6]);
-  if (eng == kEngStream) return launch_gn_fwd_stream(op, st);
-  if (eng == kEngDirect) return launch_gn_fwd_grid2(op, st);
   static DeviceOnce set;
   if (set.needed()) {
     if (int rc = gng_prepare(gn_fwd_grid_kernel)) return rc;
@@ -494,9 +466,7 @@ int launch_gn_bwd_grid(const CgdOp& op, cudaStream_t st) {
   CGD_CHECK_ARG(ld_dy % 8 == 0 && ldx % 8 == 0 && ld_dx % 8 == 0 && op.p[0] && op.p[1] && op.p[2] && op.p[3] && op.p[4] && op.p[6] && op.p[7] &&
                     op.p[8],
                 "gn_bwd_grid: bad args");
-  const int eng = gng_engine(true, N, HW, C, op.i[7]);
-  if (eng == kEngStream) return launch_gn_bwd_stream(op, st);
-  if (eng == kEngDirect) return launch_gn_bwd_grid2(op, st);
+  if (gn_bwd_direct(HW, C)) return launch_gn_bwd_grid2(op, st);
   static DeviceOnce set;
   if (set.needed()) {
     if (int rc = gng_prepare(gn_bwd_grid_kernel)) return rc;

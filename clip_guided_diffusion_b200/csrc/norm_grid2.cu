@@ -1,6 +1,6 @@
-// norm_grid2.cu -- GroupNorm(32) (+SiLU, +scale/shift) forward and input-gradient for LARGE activations, second version of
-// the single persistent launch of norm_grid.cu: same contract (ops GN_FWD_GRID / GN_BWD_GRID, same partials / barrier / stats
-// buffers), different engine.
+// norm_grid2.cu -- GroupNorm(32) (+SiLU, +scale/shift) input-gradient for LARGE activations, second version of the single
+// persistent launch of norm_grid.cu: same contract (op GN_BWD_GRID, same partials / barrier / stats buffers), different engine,
+// taken for the backward launches with HW * C >= 2^23 (norm_grid.cu, gn_bwd_direct).
 //
 // Why: the ring kernel's consumers are a latency-bound instruction stream, not a memory-bound one: one 16-byte vector per loop trip with a serial
 // HADD2 -> FFMA -> FMUL -> MUFU.EX2 -> FADD -> MUFU.RCP -> FMUL -> F2FP -> STG chain (85 SASS instructions per vector in
@@ -9,7 +9,7 @@
 // coefficients live in registers, and U vectors are in flight per thread per trip (U x 16 KB per SM).
 // Requires C % 256 == 0 (a thread's 8 channels never straddle a group); other widths keep the ring kernels.
 //
-// Replaces [3P] guided-diffusion GroupNorm32 + SiLU + scale-shift and their autograd (SURVEY.md K5, K6).
+// Replaces the autograd of [3P] guided-diffusion GroupNorm32 + SiLU + scale-shift (SURVEY.md K5, K6).
 #include "common.cuh"
 #include "ops.cuh"
 #include "pdl.cuh"
@@ -109,195 +109,6 @@ __device__ __forceinline__ void g2_sweep(int p0, int p1, int pl, int PP, L&& loa
     load(p, 0);
     f(p, 0);
   }
-}
-
-// ------------------------------------------------------------------------------------------------ forward
-template <int U>
-__global__ void __launch_bounds__(kG2Threads, 1)
-gn_fwd_grid2_kernel(const __half* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
-                    const float* __restrict__ emb, __half* __restrict__ y, float* __restrict__ stats, float* __restrict__ partials,
-                    unsigned int* __restrict__ bar, int HW, int C, int64_t ldx, int64_t ldy, int Gn, float eps, int silu) {
-  __shared__ float red_s[kG2Threads], red_q[kG2Threads];
-  __shared__ float gs[32], gq[32], fa[32], fb[32], s_mean[32], s_rstd[32];
-  const int n = blockIdx.x / Gn, chunk = blockIdx.x % Gn;
-  const int V = C / 8, PP = kG2Threads / V, cpg = C / 32, vpg = cpg / 8;
-  const int ppc = (HW + Gn - 1) / Gn;
-  const int p0 = min(HW, chunk * ppc), p1 = min(HW, p0 + ppc);
-  const int col = threadIdx.x % V, pl = threadIdx.x / V;
-  const bool active = pl < PP;
-  const int pend = active ? p1 : p0;  // idle threads (1024 % V != 0) sweep an empty range
-  pdl_wait();
-  pdl_launch_dependents();
-  const __half* xb = x + (int64_t)n * HW * ldx + col * 8;
-  uint4 v[U];
-  float2 s[4], q[4];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) s[j] = q[j] = make_float2(0.f, 0.f);
-  g2_sweep<U>(
-      p0, pend, pl, PP, [&](int p, int u) { v[u] = g2_ld(xb + (int64_t)p * ldx); },
-      [&](int, int u) {
-        float2 f[4];
-        g2_unpack(v[u], f);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          s[j] = add2(s[j], f[j]);
-          q[j] = fma2(f[j], f[j], q[j]);
-        }
-      });
-  const float ts = ((s[0].x + s[0].y) + (s[1].x + s[1].y)) + ((s[2].x + s[2].y) + (s[3].x + s[3].y));
-  const float tq = ((q[0].x + q[0].y) + (q[1].x + q[1].y)) + ((q[2].x + q[2].y) + (q[3].x + q[3].y));
-  g2_block_reduce(ts, tq, V, PP, vpg, active, red_s, red_q, gs, gq);
-  if (threadIdx.x < 32) {
-    float* o = partials + (((int64_t)n * Gn + chunk) * 32 + threadIdx.x) * 2;
-    o[0] = gs[threadIdx.x];
-    o[1] = gq[threadIdx.x];
-  }
-  g2_grid_barrier(bar, gridDim.x);
-  g2_fold(partials + (int64_t)n * Gn * 64, Gn, fa, fb);
-  if (threadIdx.x < 32) {
-    const float inv_m = 1.f / ((float)cpg * (float)HW);
-    const float mu = fa[threadIdx.x] * inv_m;
-    const float var = fmaxf(fmaf(-mu, mu, fb[threadIdx.x] * inv_m), 0.f);  // E[x^2] - mean^2: relative error ~ 6e-8 * mean^2 / var
-    const float rs = 1.f / sqrtf(var + eps);
-    s_mean[threadIdx.x] = mu;
-    s_rstd[threadIdx.x] = rs;
-    if (chunk == 0) {
-      stats[((int64_t)n * 32 + threadIdx.x) * 2 + 0] = mu;
-      stats[((int64_t)n * 32 + threadIdx.x) * 2 + 1] = rs;
-    }
-  }
-  __syncthreads();
-  float2 A[4], Bc[4];
-  {
-    const int g = min(col / vpg, 31);
-    const float mu = s_mean[g], rs = s_rstd[g];
-    float a[8], b[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int c = col * 8 + j;
-      const float ga = gamma[c], be = beta[c];
-      float sc1 = 1.f, sh = 0.f;
-      if (emb) {
-        sc1 = 1.f + emb[(int64_t)n * 2 * C + c];
-        sh = emb[(int64_t)n * 2 * C + C + c];
-      }
-      a[j] = rs * ga * sc1;
-      b[j] = (be - mu * rs * ga) * sc1 + sh;
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      A[j] = make_float2(a[2 * j], a[2 * j + 1]);
-      Bc[j] = make_float2(b[2 * j], b[2 * j + 1]);
-    }
-  }
-  __half* yb = y + (int64_t)n * HW * ldy + col * 8;
-  g2_sweep<U>(
-      p0, pend, pl, PP, [&](int p, int u) { v[u] = g2_ld(xb + (int64_t)p * ldx); },
-      [&](int p, int u) {
-        float2 f[4];
-        g2_unpack(v[u], f);
-        uint4 o;
-        uint32_t* ow = reinterpret_cast<uint32_t*>(&o);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float2 t = fma2(f[j], A[j], Bc[j]);
-          if (silu) t = silu2(t);
-          ow[j] = g2_f2h(t);
-        }
-        *reinterpret_cast<uint4*>(yb + (int64_t)p * ldy) = o;
-      });
-}
-
-// ------------------------------------------------------------------------------------------------ forward from conv-epilogue statistics
-// GN_APPLY_EPI: the conv that produced x already reduced it to per (128-pixel tile, 8-channel octet) sums (CONV flags 2,
-// conv_tc.cu, CONV flags 2), so the forward is ONE streaming trip: every CTA folds the partial sums of its image (warp g = group g, fixed
-// order, compensated fp32 -- bit-identical in every CTA, no grid barrier), then applies.  partials: [N * tpi][octs][2], tpi = HW / 128.
-template <int U>
-__global__ void __launch_bounds__(kG2Threads, 1)
-gn_apply_epi_kernel(const __half* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ emb,
-                    __half* __restrict__ y, float* __restrict__ stats, const float* __restrict__ partials, int HW, int C, int64_t ldx, int64_t ldy,
-                    int Gn, int octs, int oct0, float eps, int silu) {
-  __shared__ float s_mean[32], s_rstd[32];
-  const int n = blockIdx.x / Gn, chunk = blockIdx.x % Gn;
-  const int V = C / 8, PP = kG2Threads / V, cpg = C / 32, vpg = cpg / 8;
-  const int ppc = (HW + Gn - 1) / Gn;
-  const int p0 = min(HW, chunk * ppc), p1 = min(HW, p0 + ppc);
-  const int col = threadIdx.x % V, pl = threadIdx.x / V;
-  const bool active = pl < PP;
-  const int pend = active ? p1 : p0;
-  pdl_wait();
-  pdl_launch_dependents();
-  {
-    const int g = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int tpi = HW / 128, cnt = tpi * vpg;  // group g: octets [oct0 + g * vpg, + vpg) of every tile of image n
-    float sa = 0.f, ca = 0.f, sb = 0.f, cb = 0.f;
-    for (int m = lane; m < cnt; m += 32) {
-      const int tile = m / vpg, o = m - tile * vpg;
-      const float2 v = __ldcg(reinterpret_cast<const float2*>(partials + (((int64_t)n * tpi + tile) * octs + oct0 + g * vpg + o) * 2));
-      float t = sa + v.x;
-      ca += fabsf(sa) >= fabsf(v.x) ? (sa - t) + v.x : (v.x - t) + sa;
-      sa = t;
-      t = sb + v.y;
-      cb += fabsf(sb) >= fabsf(v.y) ? (sb - t) + v.y : (v.y - t) + sb;
-      sb = t;
-    }
-    float da = sa + ca, db = sb + cb;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      da += __shfl_xor_sync(0xffffffffu, da, o);
-      db += __shfl_xor_sync(0xffffffffu, db, o);
-    }
-    if (lane == 0) {
-      const float inv_m = 1.f / ((float)cpg * (float)HW);
-      const float mu = da * inv_m;
-      const float var = fmaxf(fmaf(-mu, mu, db * inv_m), 0.f);
-      const float rs = 1.f / sqrtf(var + eps);
-      s_mean[g] = mu;
-      s_rstd[g] = rs;
-      if (chunk == 0) {
-        stats[((int64_t)n * 32 + g) * 2 + 0] = mu;
-        stats[((int64_t)n * 32 + g) * 2 + 1] = rs;
-      }
-    }
-  }
-  __syncthreads();
-  float2 A[4], Bc[4];
-  {
-    const int g = min(col / vpg, 31);
-    const float mu = s_mean[g], rs = s_rstd[g];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float a[2], b[2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int c = col * 8 + 2 * j + h;
-        const float ga = gamma[c], be = beta[c];
-        const float sc1 = emb ? 1.f + emb[(int64_t)n * 2 * C + c] : 1.f, sh = emb ? emb[(int64_t)n * 2 * C + C + c] : 0.f;
-        a[h] = rs * ga * sc1;
-        b[h] = (be - mu * rs * ga) * sc1 + sh;
-      }
-      A[j] = make_float2(a[0], a[1]);
-      Bc[j] = make_float2(b[0], b[1]);
-    }
-  }
-  const __half* xb = x + (int64_t)n * HW * ldx + col * 8;
-  __half* yb = y + (int64_t)n * HW * ldy + col * 8;
-  uint4 v[U];
-  g2_sweep<U>(
-      p0, pend, pl, PP, [&](int p, int u) { v[u] = g2_ld(xb + (int64_t)p * ldx); },
-      [&](int p, int u) {
-        float2 f[4];
-        g2_unpack(v[u], f);
-        uint4 o;
-        uint32_t* ow = reinterpret_cast<uint32_t*>(&o);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float2 t = fma2(f[j], A[j], Bc[j]);
-          if (silu) t = silu2(t);
-          ow[j] = g2_f2h(t);
-        }
-        *reinterpret_cast<uint4*>(yb + (int64_t)p * ldy) = o;
-      });
 }
 
 // ------------------------------------------------------------------------------------------------ backward
@@ -402,47 +213,9 @@ gn_bwd_grid2_kernel(const __half* __restrict__ dy, const __half* __restrict__ x,
 }
 
 // ------------------------------------------------------------------------------------------------ host
-constexpr int kG2FwdU = 4, kG2BwdU = 2;
+constexpr int kG2BwdU = 2;
 
 bool gn_grid2_supports(int64_t C) { return C % 256 == 0 && C <= 2048; }
-
-int launch_gn_apply_epi_stream(const CgdOp& op, cudaStream_t st);  // norm_stream.cu: fold launch + streaming apply launch
-static bool epi_use_stream(const CgdOp& op) {
-  static int off = -1;
-  if (off < 0) {
-    const char* e = getenv("CGD_GN_GRID_ENGINE");
-    off = (e && e[0] == 's') ? 0 : 1;  // streaming engine opt-in
-  }
-  return !off && op.p[7] != nullptr;
-}
-int gn_apply_epi_num_launches(const CgdOp& op) { return epi_use_stream(op) ? 2 : 1; }
-
-int launch_gn_apply_epi(const CgdOp& op, cudaStream_t st) {
-  const int64_t N = op.i[0], HW = op.i[1], C = op.i[2], ldx = op.i[3], ldy = op.i[4], Gn = op.i[5], octs = op.i[6], oct0 = op.i[7];
-  CGD_CHECK_ARG(N > 0 && HW > 0 && HW % 128 == 0 && gn_grid2_supports(C) && Gn >= 1 && ldx % 8 == 0 && ldy % 8 == 0 && octs >= oct0 + C / 8 && oct0 >= 0,
-                "gn_apply_epi: bad dims (HW %% 128, C %% 256, octets)");
-  CGD_CHECK_ARG(op.p[0] && op.p[1] && op.p[2] && op.p[4] && op.p[5] && op.p[6], "gn_apply_epi: null pointer");
-  if (epi_use_stream(op)) return launch_gn_apply_epi_stream(op, st);
-  CGD_CUDA(launch_pdl(gn_apply_epi_kernel<kG2FwdU>, dim3((unsigned)(N * Gn)), dim3(kG2Threads), 0, st, (const __half*)op.p[0], (const float*)op.p[1],
-                      (const float*)op.p[2], (const float*)op.p[3], (__half*)op.p[4], (float*)op.p[5], (const float*)op.p[6], (int)HW, (int)C, ldx, ldy,
-                      (int)Gn, (int)octs, (int)oct0, op.f[0], (int)(op.flags & 1)));
-  return 0;
-}
-
-int launch_gn_fwd_grid2(const CgdOp& op, cudaStream_t st) {
-  const int64_t N = op.i[0], HW = op.i[1], C = op.i[2], ldx = op.i[3], ldy = op.i[4], Gn = op.i[5];
-  static DeviceOnce checked;
-  if (checked.needed()) {
-    int occ = 0;
-    CGD_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, gn_fwd_grid2_kernel<kG2FwdU>, kG2Threads, 0));
-    CGD_CHECK_ARG(occ >= 1, "gn_fwd_grid2: the 1024-thread CTA does not fit an SM (occupancy %d)", occ);
-    checked.mark();
-  }
-  CGD_CUDA(launch_pdl(gn_fwd_grid2_kernel<kG2FwdU>, dim3((unsigned)(N * Gn)), dim3(kG2Threads), 0, st, (const __half*)op.p[0],
-                      (const float*)op.p[1], (const float*)op.p[2], (const float*)op.p[3], (__half*)op.p[4], (float*)op.p[5], (float*)op.p[6],
-                      (unsigned int*)op.p[7], (int)HW, (int)C, ldx, ldy, (int)Gn, op.f[0], (int)(op.flags & 1)));
-  return 0;
-}
 
 int launch_gn_bwd_grid2(const CgdOp& op, cudaStream_t st) {
   const int64_t N = op.i[0], HW = op.i[1], C = op.i[2], ld_dy = op.i[3], ldx = op.i[4], ld_dx = op.i[5], Gn = op.i[6];

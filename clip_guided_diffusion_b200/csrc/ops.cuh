@@ -28,9 +28,6 @@ int launch_copy(const CgdOp& op, cudaStream_t st);
 int launch_attn_fwd(const CgdOp& op, cudaStream_t st);
 int launch_attn_bwd(const CgdOp& op, cudaStream_t st);
 int attn_bwd_num_launches(const CgdOp& op);
-int launch_transpose(const CgdOp& op, cudaStream_t st);
-int launch_softmax_fwd(const CgdOp& op, cudaStream_t st);
-int launch_softmax_bwd(const CgdOp& op, cudaStream_t st);
 int launch_linear_small(const CgdOp& op, cudaStream_t st);
 int launch_timestep_emb(const CgdOp& op, cudaStream_t st);
 int launch_label_add(const CgdOp& op, cudaStream_t st);
@@ -49,9 +46,6 @@ int launch_seed_quant(const CgdOp& op, cudaStream_t st);
 int launch_mag_clamp(const CgdOp& op, cudaStream_t st);
 int launch_attnpool_embed_fwd(const CgdOp& op, cudaStream_t st);
 int launch_attnpool_embed_bwd(const CgdOp& op, cudaStream_t st);
-int launch_gn_apply_epi(const CgdOp& op, cudaStream_t st);
-int gn_grid_num_launches(const CgdOp& op);
-int gn_apply_epi_num_launches(const CgdOp& op);
 int launch_spherical(const CgdOp& op, cudaStream_t st);
 int launch_pmv_blend(const CgdOp& op, cudaStream_t st);
 int launch_guide_grad(const CgdOp& op, cudaStream_t st);

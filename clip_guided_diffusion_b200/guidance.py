@@ -149,7 +149,7 @@ class EngineModel:
             raise RuntimeError(f"Error(s) in loading state_dict: missing {missing[:4]}{'...' if len(missing) > 4 else ''}, "
                                f"unexpected {unexpected[:4]}{'...' if len(unexpected) > 4 else ''}")
         shadow = Plan(conv_impl=eng.plan.conv_impl)
-        for flag in ("grid_gn", "fused_gn", "tc_attention", "cluster_splitk", "gn_epi_stats"):
+        for flag in ("grid_gn", "fused_gn", "cluster_splitk"):
             setattr(shadow, flag, getattr(eng.plan, flag))
         UNetB200(eng.unet.cfg, state_dict, batch=eng.B, height=eng.H, width=eng.W, device="cpu", seed_scale=eng.unet.seed_scale, plan=shadow,
                  build_backward=eng.vit is not None)

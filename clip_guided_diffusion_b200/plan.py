@@ -201,13 +201,6 @@ def gn_fused_cluster(N: int, HW: int, C: int, maxv: int) -> int:
 
 
 N_SMS = 132  # H100 SXM
-GN_STREAM_CTAS = 132 * 8  # partial-sum slots of the streaming GroupNorm engine (csrc/norm_stream.cu: kGsMaxCtas)
-
-
-def gn_partial_floats(N: int, gn_g: int) -> int:
-    """partials buffer of a GN_*_GRID op: room for the persistent engines (N * Gn rows of 64 floats) and for the streaming engine
-    (up to GN_STREAM_CTAS rows + the folded sums)"""
-    return max(N * gn_g, GN_STREAM_CTAS) * 64 + N * 64
 
 
 def gn_grid_ctas(N: int, HW: int, C: int) -> int:
@@ -230,19 +223,12 @@ class Plan:
         self._tape: list[Callable[[], None]] = []
         self._grads: dict = {}
         self.conv_impl = conv_impl
-        # long sequences (T % 256 == 0) as batched tensor-core GEMMs + transposes + softmax kernels; superseded by the flash kernels of
-        # csrc/attention_mma.cu (one launch forward, three backward, nothing T x T in HBM), kept for A/B measurements
-        self.tc_attention = os.environ.get("CGD_TC_ATTENTION", "0") == "1"
         # split-K reduced inside a thread-block cluster through DSMEM (csrc/conv_tc.cu) instead of partials + a reduce launch
         self.cluster_splitk = os.environ.get("CGD_CONV_CLUSTER", "1") == "1"
         # ... also for one-wave layers that did not need split-K to fill the machine but have long K loops (the 64 x 64 level's
         # 512 -> 512 and 1024 -> 512 3x3s): a wider tile split along K inside a cluster shortens the K loop per SM.
         # CGD_CLUSTER_WIDE=0 switches it off for A/B runs.
         self.cluster_wide = os.environ.get("CGD_CLUSTER_WIDE", "1") == "1"
-        # GroupNorm forward from statistics reduced in the producing conv's epilogue (CONV flags 2 + GN_APPLY_EPI): one streaming trip
-        # instead of two.  Interpreter-verified, NOT yet run on the device: opt-in until it is (DESIGN.md "Next")
-        self.gn_epi_stats = os.environ.get("CGD_GN_EPI_STATS", "0") == "1"
-        self._epi_stats = {}  # output Act key -> (partials Buf, octets per tile row)
         self._gelu_src = {}   # QuickGELU output Act key -> its pre-activation Act (dgrad-epilogue fusion, CONV flags 4)
         self.arena: Optional[th.Tensor] = None
         self.handle = None
@@ -320,23 +306,21 @@ class Plan:
 
     # ------------------------------------------------------------------ conv / GEMM
     def _emit_conv(self, x_ptr, x_strides, NB, H, W, Cin, wbuf, npad, Cout, taps, bias, res_ptr, res_strides, out_ptr, out_strides,
-                   out_f32=False, out_sc=1, tag="", b_ptr=None, b_batch=(0, 0), ldb=0, want_stats=False, res_gelu=False):
-        """b_ptr / b_batch / ldb: batched-GEMM mode (attention): the B operand is a strided activation matrix selected by the
-        tile's (h, n) instead of a packed weight."""
+                   out_f32=False, out_sc=1, tag="", res_gelu=False):
         m_tiles = conv_tile_count(NB, H, W)
         kblocks = taps * Cin // 64
         bn = pick_bn(npad, m_tiles, kblocks)
         splits = pick_splits(m_tiles, npad // bn, kblocks, npad)
         cluster = 0
-        if splits > 1 and self.cluster_splitk and self.conv_impl in (0, 3) and b_ptr is None and not out_f32 and out_sc == 1:
+        if splits > 1 and self.cluster_splitk and self.conv_impl in (0, 3) and not out_f32 and out_sc == 1:
             # one launch and no fp32 partial tensor, unless the workspace split would give each CTA a shorter K loop
             pick = pick_cluster_split(m_tiles, npad, kblocks, Cout)
             if pick is not None and pick[2] <= -(-kblocks // splits):
                 bn, splits = pick[:2]
                 cluster = 1
-        elif (splits == 1 and self.cluster_wide and self.cluster_splitk and self.conv_impl in (0, 3) and b_ptr is None and not out_f32 and out_sc == 1
+        elif (splits == 1 and self.cluster_wide and self.cluster_splitk and self.conv_impl in (0, 3) and not out_f32 and out_sc == 1
               and not res_gelu  # the QuickGELU' epilogue needs splits == 1 (conv_gelu_epilogue_ok)
-              and m_tiles >= 2 and kblocks >= 32 and not (want_stats and self.gn_epi_stats)):
+              and m_tiles >= 2 and kblocks >= 32):
             # one wave of narrow tiles with a long K loop (the 64 x 64 level: 64 BN-128 tiles x 72 K-blocks = 33 us at 0.46 us per K-block):
             # wider tiles split along K inside a cluster can be shorter even though no split-K was "needed" to fill the machine
             pick = pick_cluster_split(m_tiles, npad, kblocks, Cout)
@@ -348,23 +332,11 @@ class Plan:
         if splits > 1 and not cluster:
             ws = self.new(splits * m_tiles * 128 * npad, "f", "splitk_ws")
         i = [NB, H, W, Cin, Cout, npad, taps, *x_strides, *out_strides, *(res_strides or (0, 0, 0)), bn, splits, self.conv_impl, out_sc,
-             b_batch[0], b_batch[1], ldb, cluster]
-        # epilogue statistics for a following GroupNorm: tensor-core kernel without split-K, full 128-pixel tiles inside an image
-        stats = None
-        tw = 1
-        while tw < W and tw < 128:
-            tw <<= 1
-        t_h = min(128 // tw, 1 << max(0, (H - 1).bit_length()))
-        if (want_stats and self.gn_epi_stats and self.conv_impl in (0, 3) and splits == 1 and not cluster and not out_f32 and out_sc == 1 and b_ptr is None
-                and bn >= 64 and Cout % 64 == 0 and m_tiles >= 2 and m_tiles % 2 == 0 and tw * t_h == 128 and W % tw == 0 and H % t_h == 0
-                and (tw == W or t_h == 1)):
-            stats = self.new(m_tiles * (npad // 8) * 2, "f", "epi_stats")
+             0, 0, 0, cluster]  # i20..i22 reserved
         if res_gelu:
             assert self.conv_gelu_epilogue_ok(NB, H, W, Cin, npad, Cout, taps), tag
-        self.emit("CONV", flags=(1 if out_f32 else 0) | (2 if stats is not None else 0) | (4 if res_gelu else 0), i=i,
-                  p=[x_ptr, b_ptr if b_ptr is not None else self._bp(wbuf), self._bp(bias), res_ptr, out_ptr, self._bp(ws), None]
-                  + ([self._bp(stats)] if stats is not None else []), tag=tag)
-        return stats
+        self.emit("CONV", flags=(1 if out_f32 else 0) | (4 if res_gelu else 0), i=i,
+                  p=[x_ptr, self._bp(wbuf), self._bp(bias), res_ptr, out_ptr, self._bp(ws), None], tag=tag)
 
     def conv_gelu_epilogue_ok(self, NB, H, W, Cin, npad, Cout, taps) -> bool:
         """would this conv run with the epilogue that implements CONV flags 4?  Mirrors the choices of `_emit_conv` /
@@ -376,15 +348,6 @@ class Plan:
         bn = pick_bn(npad, m_tiles, kblocks)
         return (m_tiles >= 2 or self.conv_impl == 3) and pick_splits(m_tiles, npad // bn, kblocks, npad) == 1 and bn >= 64 and Cout % 64 == 0
 
-    def _gn_would_use_epi(self, y: Act) -> bool:
-        """would a GroupNorm over y take the statistics of the producing conv's epilogue?  (the large activations of the persistent
-        grid kernels; the small ones keep the one-launch cluster kernel)"""
-        if not self.gn_epi_stats or y.HW % 128 or y.C % 256:
-            return False
-        if self.fused_gn and gn_fused_cluster(y.N, y.HW, y.C, 16):
-            return False
-        return bool(self.grid_gn and gn_grid_ctas(y.N, y.HW, y.C))
-
     @staticmethod
     def _strides(a: Act):
         return (a.H * a.W * a.ld, a.W * a.ld, a.ld)
@@ -394,11 +357,8 @@ class Plan:
         assert x.C == w.cin_pad, (x.C, w.cin_pad, name)
         y = out if out is not None else self.act(x.N, x.H, x.W, w.cout, name)
         assert y.C == w.cout and (y.N, y.H, y.W) == (x.N, x.H, x.W)
-        stats = self._emit_conv(self._ap(x), self._strides(x), x.N, x.H, x.W, x.C, w.fwd, w.fwd_npad, w.cout, w.taps, w.bias,
-                                self._ap(res), self._strides(res) if res is not None else None, self._ap(y), self._strides(y), tag=name,
-                                want_stats=self._gn_would_use_epi(y))
-        if stats is not None:
-            self._epi_stats[y.key()] = (stats, w.fwd_npad // 8)
+        self._emit_conv(self._ap(x), self._strides(x), x.N, x.H, x.W, x.C, w.fwd, w.fwd_npad, w.cout, w.taps, w.bias,
+                        self._ap(res), self._strides(res) if res is not None else None, self._ap(y), self._strides(y), tag=name)
 
         def bwd():
             dy = self.grad_of(y)
@@ -437,18 +397,13 @@ class Plan:
         embp = self._bp(emb[0], emb[1]) if emb is not None else None
         cs_f = gn_fused_cluster(N, HW, C, 16) if self.fused_gn else 0
         gn_g = gn_grid_ctas(N, HW, C) if self.grid_gn else 0
-        epi = self._epi_stats.get(x.key()) if self.gn_epi_stats else None
-        if epi is not None and not cs_f and gn_g and HW % 128 == 0 and C % 256 == 0:
-            sums = self.new(N * 64, "f", name + "_sums")  # folded group sums (streaming engine: fold launch -> apply launch)
-            self.emit("GN_APPLY_EPI", flags=1 if silu else 0, i=[N, HW, C, x.ld, y.ld, gn_g, epi[1], 0], f=[eps],
-                      p=[self._ap(x), self._bp(gamma), self._bp(beta), embp, self._ap(y), self._bp(stats), self._bp(epi[0]), self._bp(sums)], tag=name)
-        elif cs_f:
+        if cs_f:
             self.emit("GN_FWD_FUSED", flags=1 if silu else 0, i=[N, HW, C, x.ld, y.ld, cs_f], f=[eps],
                       p=[self._ap(x), self._bp(gamma), self._bp(beta), embp, self._ap(y), self._bp(stats)], tag=name)
         elif gn_g:
-            partials = self.new(gn_partial_floats(N, gn_g), "f", name + "_part")
+            partials = self.new(N * gn_g * 64, "f", name + "_part")
             bar = self.new(2, "u32", name + "_bar")
-            self.emit("GN_FWD_GRID", flags=1 if silu else 0, i=[N, HW, C, x.ld, y.ld, gn_g, gn_partial_floats(N, gn_g)], f=[eps],
+            self.emit("GN_FWD_GRID", flags=1 if silu else 0, i=[N, HW, C, x.ld, y.ld, gn_g], f=[eps],
                       p=[self._ap(x), self._bp(gamma), self._bp(beta), embp, self._ap(y), self._bp(stats), self._bp(partials), self._bp(bar)], tag=name)
         else:
             pp = max(1, 256 // (C // 8))
@@ -471,12 +426,12 @@ class Plan:
             if cs_b:
                 self.emit("GN_BWD_FUSED", flags=fl, i=[N, HW, C, dy.ld, x.ld, dx.ld, cs_b], f=[eps], p=common + [self._ap(dx)], tag="d_" + name)
             elif gn_g:
-                bpart = self.new(gn_partial_floats(N, gn_g), "f", name + "_bpart")
+                bpart = self.new(N * gn_g * 64, "f", name + "_bpart")
                 bbar = self.new(2, "u32", name + "_bbar")
                 # one scratch tensor shared by every GroupNorm backward of the plan (they run one after the other)
                 if self._gn_scratch is None or self._gn_scratch.numel < N * HW * C:
                     self._gn_scratch = self.new(N * HW * C, "h", "gn_bwd_dxhat")
-                self.emit("GN_BWD_GRID", flags=fl, i=[N, HW, C, dy.ld, x.ld, dx.ld, gn_g, gn_partial_floats(N, gn_g)], f=[eps],
+                self.emit("GN_BWD_GRID", flags=fl, i=[N, HW, C, dy.ld, x.ld, dx.ld, gn_g], f=[eps],
                           p=common + [self._ap(dx), self._bp(bpart), self._bp(bbar), self._bp(self._gn_scratch)], tag="d_" + name)
             else:
                 pp = max(1, 256 // (C // 8))
@@ -604,8 +559,6 @@ class Plan:
         C = qkv.C // 3
         d = C // heads
         assert d in (64, 128, 192, 256), f"attention kernels support head dims 64 / 128 / 192 / 256, got {d}"
-        if d == 64 and T % 256 == 0 and self.tc_attention and self.conv_impl in (0, 1, 3):
-            return self._attention_tc(qkv, heads, T, nbatch, legacy_order, name)
         out = Act(self.new(nbatch * T * C, "h", name), 0, qkv.N, qkv.H, qkv.W, C, C)
         lse = self.new(nbatch * heads * T, "f", name + "_lse")
         if legacy_order:
@@ -629,62 +582,6 @@ class Plan:
             self.emit("ATTN_BWD", i=ii, f=[scale],
                       p=[q, k, v, self._ap(out), self._ap(do), self._bp(lse), (dqkv.buf, qo), (dqkv.buf, ko), (dqkv.buf, vo), self._bp(delta)],
                       tag="d_" + name)
-            self.add_grad(qkv, dqkv)
-
-        self._tape.append(bwd)
-        return out
-
-    def _attention_tc(self, qkv: Act, heads: int, T: int, B: int, legacy_order: bool, name: str) -> Act:
-        """softmax(Q K^T / sqrt(d)) V for T % 256 == 0 as batched tensor-core GEMMs (S and P materialised in fp16 like the
-        reference's einsum / softmax(w.float()).type(dtype)), transposes so that every operand is K-major, row softmax."""
-        C = qkv.C // 3
-        d, ld = 64, qkv.ld
-        hs, qo, ko, vo = (3 * d, 0, d, 2 * d) if legacy_order else (d, 0, C, 2 * C)
-        scale = 1.0 / math.sqrt(d)
-        q, k, v = ((qkv.buf, qkv.eoff + o) for o in (qo, ko, vo))
-        qkv_str = (T * ld, hs, ld)          # (batch, head, row) strides of a q / k / v view
-        tt_str = (heads * T * T, T * T, T)  # [B, heads, T, T] matrices
-        dt_str = (d * T, heads * d * T)     # per-head / per-batch strides of [B, heads, d, T] transposes
-        out = Act(self.new(B * T * C, "h", name), 0, qkv.N, qkv.H, qkv.W, C, C)
-        o_str = (T * C, d, C)
-        S = self.new(B * heads * T * T, "h", name + "_P")
-        lse = self.new(B * heads * T, "f", name + "_lse")
-        Vt = self.new(B * heads * d * T, "h", name + "_Vt")
-        rows = B * heads * T
-
-        def gemm(a_ptr, a_str, K, b_ptr, b_ld, b_batch, N, o_ptr, o_strides, tag):
-            self._emit_conv(a_ptr, a_str, B, heads, T, K, None, N, N, 1, None, None, None, o_ptr, o_strides, tag=tag,
-                            b_ptr=b_ptr, b_batch=b_batch, ldb=b_ld)
-
-        def transpose(pairs, R, Cc, tag):
-            ii = [B, heads, R, Cc] + [0] * 9 + [R]
-            pp = []
-            for j, (src, sstr, dst) in enumerate(pairs):
-                ii[4 + 3 * j: 7 + 3 * j] = list(sstr)
-                pp += [src, (dst, 0)]
-            self.emit("TRANSPOSE", i=ii, p=pp, tag=tag)
-
-        transpose([(v, qkv_str, Vt)], T, d, name + ".Vt")
-        gemm(q, qkv_str, d, k, ld, (hs, T * ld), T, (S, 0), tt_str, name + ".QK^T")
-        self.emit("SOFTMAX_FWD", i=[rows, T, T], f=[scale], p=[(S, 0), (lse, 0)], tag=name + ".softmax")
-        gemm((S, 0), tt_str, T, (Vt, 0), T, dt_str, d, self._ap(out), o_str, name + ".PV")
-
-        def bwd():
-            do = self.grad_of(out)
-            if do is None:
-                return
-            assert do.ld == C
-            dOt, Kt, Qt = (self.new(B * heads * d * T, "h", name + n_) for n_ in ("_dOt", "_Kt", "_Qt"))
-            transpose([(self._ap(do), o_str, dOt), (k, qkv_str, Kt), (q, qkv_str, Qt)], T, d, "d_" + name + ".T1")
-            dP = self.new(B * heads * T * T, "h", name + "_dS")
-            gemm(self._ap(do), o_str, d, v, ld, (hs, T * ld), T, (dP, 0), tt_str, "d_" + name + ".dP")
-            self.emit("SOFTMAX_BWD", i=[rows, T, T], f=[scale], p=[(S, 0), (dP, 0)], tag="d_" + name + ".softmax")
-            Pt, dSt = (self.new(B * heads * T * T, "h", name + n_) for n_ in ("_Pt", "_dSt"))
-            transpose([((S, 0), tt_str, Pt), ((dP, 0), tt_str, dSt)], T, T, "d_" + name + ".T2")
-            dqkv = Act(self.new(B * T * ld, "h", "d_" + name), 0, qkv.N, qkv.H, qkv.W, qkv.C, ld)
-            gemm((Pt, 0), tt_str, T, (dOt, 0), T, dt_str, d, (dqkv.buf, vo), qkv_str, "d_" + name + ".dV")
-            gemm((dP, 0), tt_str, T, (Kt, 0), T, dt_str, d, (dqkv.buf, qo), qkv_str, "d_" + name + ".dQ")
-            gemm((dSt, 0), tt_str, T, (Qt, 0), T, dt_str, d, (dqkv.buf, ko), qkv_str, "d_" + name + ".dK")
             self.add_grad(qkv, dqkv)
 
         self._tape.append(bwd)

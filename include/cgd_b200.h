@@ -33,7 +33,9 @@
 extern "C" {
 #endif
 
-#define CGD_ABI_VERSION 2  /* 2: CONV i23 clusters of `splits` CTAs (were 2 * splits), p6 unused, i18 = 3 no longer the narrow kernels */
+#define CGD_ABI_VERSION 3  /* 3: op codes 30, 31, 32, 49 retired; CONV i20..i22 and flags 2 reserved (must be 0); GN_*_GRID without the
+                              partials-capacity operand (GN_FWD_GRID i6, GN_BWD_GRID i7)
+                              2: CONV i23 clusters of `splits` CTAs (were 2 * splits), p6 unused, i18 = 3 no longer the narrow kernels */
 #define CGD_OP_NI 24
 #define CGD_OP_NF 8
 #define CGD_OP_NP 12
@@ -57,16 +59,14 @@ enum {
    *   p0 A(h)  p1 Wp(h, [Npad, taps*Cin] K-major)  p2 bias(f)|0  p3 res(h)|0  p4 out(h|f)  p5 splitK ws(f)|0
    *   i0 NB i1 H i2 W i3 Cin(%64==0) i4 Cout i5 Npad(%BN==0) i6 taps(1|9)
    *   i7..9 A strides (n,h,w)  i10..12 out strides  i13..15 res strides  i16 BN  i17 splits
-   *   i18 impl (0 = wgmma, with the mma.sync kernels for narrow / 8x8 layers; 1 = SIMT verification kernel; 2 = the wgmma tile kernel for
+   *   i18 impl (0 = wgmma, with the mma.sync kernel for narrow layers; 1 = SIMT verification kernel; 2 = the wgmma tile kernel for
    *   every layer, workspace split-K only; 3 = the wgmma tile kernel for every layer, with in-cluster split-K and the fused epilogues)  i19 out channel stride (0/1 = contiguous; >1 only
    *   with scalar stores, e.g. fp32 NCHW outputs of the UNet head / stem dgrad)
-   *   i20, i21 batched-GEMM mode: element strides of the B operand per h / per n index (0, 0 = one shared weight matrix);
-   *   i22 row stride of B (0 = taps*Cin).  Batched mode needs W > 64, one (h, n) per 128-pixel tile (attention: A = Q/P/dS..., B = K/V^T/...)
+   *   i20, i21, i22 reserved (0)
    *   p6 unused (0)
    *   i23 = 1: split-K inside a thread-block cluster of `splits` CTAs, reduced through distributed shared memory (one launch, no
    *   workspace; splits in 2..8, BN >= 64, BN / splits a multiple of 16, fp16 contiguous output, Cout % 8 == 0)
-   *   flags: 1 = out is fp32 ; 2 = epilogue statistics for CGD_OP_GN_APPLY_EPI into p7 (wgmma kernel, no split-K, fp16 output, full
-   *   128-pixel tiles inside one image) ; 4 = p3 is a QuickGELU pre-activation u and out = acc * QuickGELU'(u) instead of acc + res
+   *   flags: 1 = out is fp32 ; 2 reserved (0) ; 4 = p3 is a QuickGELU pre-activation u and out = acc * QuickGELU'(u) instead of acc + res
    *   (dgrad of the CLIP MLP's c_proj writing d c_fc directly; wgmma kernel, no split-K, Cout % 8 == 0, no bias) */
   CGD_OP_CONV = 1,
   /* GroupNorm(32) statistics: per (image, chunk, group) partial sum / sum of squares; the last block per image
@@ -166,16 +166,7 @@ enum {
   CGD_OP_SAMPLE_DDIM = 28,
   /* fp16 copy of a [rows, C] block: p0 src p1 dst ; i0 rows i1 C i2 lds i3 ldd */
   CGD_OP_COPY = 29,
-  /* batched fp16 transpose, up to three (src, dst) pairs per launch: dst[b1][b2][c][r] = src[b1][b2][r][c]
-   * p0 src0 p1 dst0 p2 src1 p3 dst1 p4 src2 p5 dst2 (unused pairs null) ; i0 nb1 i1 nb2 i2 R i3 C
-   * i4..6 src0 strides (b1, b2, row)  i7..9 src1  i10..12 src2 ; i13 Rp (dst row stride; dst dense [nb1][nb2][C][Rp]) */
-  CGD_OP_TRANSPOSE = 30,
-  /* row softmax in place: S (fp16 un-scaled logits [rows, Tp]) -> P = softmax(f0 * S[:, :T]) ; p1 lse(f [rows])|0
-   * p0 S ; i0 rows i1 T i2 Tp ; f0 scale.  With CGD_OP_CONV (batched B) this is the tensor-core attention of the
-   * 32x32 / 16x16 UNet levels ([3P] QKVAttention(Legacy): softmax(w.float()).type(w.dtype); SURVEY K4). */
-  CGD_OP_SOFTMAX_FWD = 31,
-  /* softmax backward in place on dP: dS = P * (dP - rowsum(P * dP)) * f0 ; p0 P p1 dP ; i0 rows i1 T i2 Tp */
-  CGD_OP_SOFTMAX_BWD = 32,
+  /* 30, 31, 32 retired (batched-GEMM attention: TRANSPOSE, SOFTMAX_FWD, SOFTMAX_BWD); not to be reused */
   /* single-launch GroupNorm(32) forward for activations whose (image, group) slab fits one thread-block cluster's
    * registers (C % 256 == 0, ceil(HW / CS) <= 16 * 512 / vectors-per-pixel): exact two-pass statistics exchanged through
    * distributed shared memory, y = silu?( GN(x)*(1+scale)+shift ), stats written for the backward.
@@ -189,14 +180,11 @@ enum {
   /* single persistent launch for LARGE activations: statistics pass, grid-wide barrier (generation counted, no reset needed),
    * apply pass over the same pixel range (L2 hit).  One 512-thread CTA per SM: N * Gn must not exceed the SM count.
    * p0 x(h) p1 gamma p2 beta p3 emb|0 p4 y(h) p5 stats(f [N,32,2]) p6 partials(f [N,Gn,32,2]) p7 barrier(u32 [2], zero-initialised)
-   * i0 N i1 HW i2 C i3 ldx i4 ldy i5 Gn (CTAs per image) ; f0 eps ; flags 1 = SiLU.  C % 64 == 0
-   * i6 = capacity of p6 in floats (0 = N * Gn * 64).  With C % 256 == 0 and room for N * min(1184 / N, HW / (2 * rows per CTA)) * 64
-   * + N * 64 floats the op runs as three streaming launches instead (csrc/norm_stream.cu: per-CTA partial sums, fold, apply) */
+   * i0 N i1 HW i2 C i3 ldx i4 ldy i5 Gn (CTAs per image) ; f0 eps ; flags 1 = SiLU.  C % 64 == 0 */
   CGD_OP_GN_FWD_GRID = 35,
-  /* backward of the above: p0 dy p1 x p2 stats p3 gamma p4 beta p5 emb|0 p6 dx(h) p7 partials p8 barrier
+  /* backward of the above: p0 dy p1 x p2 stats p3 gamma p4 beta p5 emb|0 p6 dx(h) p7 partials(f [N,Gn,32,2]) p8 barrier
    * p9 scratch(h, dense [N,HW,C])|0: d xhat is stored once and streamed back instead of recomputing SiLU' in the apply pass
-   * i0 N i1 HW i2 C i3 ld_dy i4 ldx i5 ld_dx i6 Gn i7 capacity of p7 in floats (see GN_FWD_GRID i6) ; flags 1 = SiLU,
-   * 2 = accumulate into dx */
+   * i0 N i1 HW i2 C i3 ld_dy i4 ldx i5 ld_dx i6 Gn ; flags 1 = SiLU, 2 = accumulate into dx */
   CGD_OP_GN_BWD_GRID = 36,
   /* y = max(x, 0) on n fp16 elements (n % 8 == 0; in place allowed): p0 x p1 y ; i0 n.  [3P] VGG16 ReLU of lpips.LPIPS (K21) */
   CGD_OP_RELU_FWD = 37,
@@ -230,13 +218,7 @@ enum {
   CGD_OP_ATTNPOOL_EMBED_FWD = 47,
   /* dx[n,t,:] (=|+=) dy[n,1+t,:] + dy[n,0,:] / HW : p0 dy(h [n,HW+1,C]) p1 dx(h, row stride i3) ; i0 n i1 HW i2 C i3 ld_dx ; flags 2 = accumulate */
   CGD_OP_ATTNPOOL_EMBED_BWD = 48,
-  /* GroupNorm(32) (+scale-shift, +SiLU) forward in ONE streaming trip from statistics the producing conv already reduced (CONV flags 2:
-   * p7 = partials(f [m_tiles][Npad/8][2]): sum / sum of squares of the fp16 output per 128-pixel tile and 8-channel octet).
-   * p0 x(h) p1 gamma p2 beta p3 emb|0 p4 y(h) p5 stats(f [N,32,2] = mean, rstd, for the backward) p6 partials
-   * i0 N i1 HW (% 128 == 0) i2 C (% 256 == 0) i3 ldx i4 ldy i5 CTAs per image i6 octets per tile row of the partials (producer Npad / 8)
-   * i7 first octet of x's channels in the producer's output ; f0 eps ; flags 1 = SiLU
-   * p7 scratch(f [N * 64])|0: when given, the op runs as a fold launch (partials -> group sums) + a streaming apply launch */
-  CGD_OP_GN_APPLY_EPI = 49,
+  /* 49 retired (GroupNorm from conv-epilogue statistics: GN_APPLY_EPI); not to be reused */
   /* MakeCutouts with use_augs=True (cgd/modules.py:12-24, 60-64): crop -> RandomHorizontalFlip -> +noise -> RandomAffine (nearest,
    * fill 0) -> +noise -> RandomPerspective (bilinear, fill 0) -> +noise -> RandomGrayscale -> +noise -> adaptive_avg_pool2d ->
    * CLIP_NORMALIZE, one gather launch; like CUTOUTS_FWD plus p3 params(f [cutn,20]: flip | inverse affine matrix[6] | perspective on |

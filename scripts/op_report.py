@@ -46,10 +46,6 @@ def shape_of(kind, op):
     return " ".join(str(v) for v in i[:6])
 
 
-# the launch list was taken with the streaming GroupNorm engine unless CGD_GN_GRID_ENGINE said otherwise (same variable as the library)
-STREAM = os.environ.get("CGD_GN_GRID_ENGINE", "direct")[0] == "s"
-
-
 def main():
     launches = load_launches(sys.argv[1])
     filt = sys.argv[2] if len(sys.argv) > 2 else None
@@ -76,10 +72,6 @@ def main():
             n = 1 if op.i[2] <= 64 and op.i[3] == 64 else 2
         elif kind == "FINAL_GRAD" and op.flags & 1:
             n = 2
-        elif kind in ("GN_FWD_GRID", "GN_BWD_GRID") and STREAM and op.i[2] % 256 == 0:
-            n = 3  # streaming engine (csrc/norm_stream.cu): partial statistics, fold, apply
-        elif kind == "GN_APPLY_EPI" and STREAM and len(op.p) > 7 and op.p[7] is not None:
-            n = 2  # fold + apply
         t = sum(v for _, v in launches[li:li + n])
         li += n
         kinds[kind][0] += 1; kinds[kind][1] += t

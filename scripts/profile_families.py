@@ -60,9 +60,9 @@ for k in sorted(step_ops, key=lambda k: -work(plan.ops[k])):
     seen.add(key)
     chosen.append(k)
 only = [v for v in os.environ.get("PF_ONLY", "").split(",") if v]
-if only:  # e.g. PF_ONLY=GN_APPLY_EPI,CONV_STATS with CGD_GN_EPI_STATS=1
+if only:
     def label(op):
-        return "CONV_STATS" if CODE[op.code] == "CONV" and (op.flags & 2) else CODE[op.code]
+        return CODE[op.code]
     chosen = [k for k in chosen if label(plan.ops[k]) in only]
     for want in only:  # make sure the biggest instance of each requested kind is there even if its key collided
         cands = [k for k in step_ops if label(plan.ops[k]) == want]

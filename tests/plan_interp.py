@@ -59,15 +59,7 @@ class Interp:
         rsn, rsh, rsw = op.i[13:16]
         osc = op.i[19] if len(op.i) > 19 and op.i[19] > 0 else 1
         A = self.V(op.p[0], (NB, H, W, Cin), (asn, ash, asw, 1)).float()
-        b_sh, b_sn, ldb = (list(op.i) + [0] * 24)[20:23]
-        ldb = ldb or taps * Cin
-        if b_sh or b_sn:  # batched GEMM: B selected per (n, h)
-            Wb = self.V(op.p[1], (NB, H, Cout, Cin), (b_sn, b_sh, ldb, 1)).float()
-            y = th.einsum("nhwk,nhck->nhwc", A, Wb)
-            out = self.V(op.p[4], (NB, H, W, Cout), (osn, osh, osw, osc))
-            out.copy_(y)
-            return
-        Wp = self.V(op.p[1], (Npad, taps * Cin), (ldb, 1)).float()[:Cout]
+        Wp = self.V(op.p[1], (Npad, taps * Cin), (taps * Cin, 1)).float()[:Cout]
         if taps == 9:
             wt = Wp.view(Cout, 3, 3, Cin).permute(0, 3, 1, 2)
             y = F.conv2d(A.permute(0, 3, 1, 2), wt, padding=1).permute(0, 2, 3, 1)
@@ -82,31 +74,7 @@ class Interp:
                 y = y * (sg * (1 + 1.702 * r * (1 - sg)))
             else:
                 y = y + r
-        out = self.V(op.p[4], (NB, H, W, Cout), (osn, osh, osw, osc))
-        out.copy_(y)
-        if op.flags & 2:  # epilogue statistics: per (128 consecutive pixels, 8-channel octet) sum / sum of squares of the STORED values
-            assert (NB * H * W) % 128 == 0 and Cout % 8 == 0
-            stored = out.float().reshape(NB * H * W // 128, 128, Cout // 8, 8)
-            part = self.V(op.p[7], (NB * H * W // 128, Npad // 8, 2), (Npad // 8 * 2, 2, 1))
-            part[:, :Cout // 8, 0] = stored.sum(dim=(1, 3))
-            part[:, :Cout // 8, 1] = stored.square().sum(dim=(1, 3))
-
-    def op_GN_APPLY_EPI(self, op):
-        N, HW, C, ldx, ldy, _, octs, oct0 = op.i[:8]
-        tpi, cpg = HW // 128, C // 32
-        part = self.V(op.p[6], (N, tpi, octs, 2), (tpi * octs * 2, octs * 2, 2, 1))[:, :, oct0:oct0 + C // 8].double()
-        tot = part.sum(dim=1).view(N, 32, cpg // 8, 2).sum(dim=2)  # [N, 32, 2]
-        mean = tot[..., 0] / (cpg * HW)
-        var = (tot[..., 1] / (cpg * HW) - mean * mean).clamp_min(0)
-        st = self.V(op.p[5], (N, 32, 2), (64, 2, 1))
-        st[:, :, 0] = mean.float()
-        st[:, :, 1] = (1.0 / th.sqrt(var.float() + op.f[0]))
-        A, Bc, _, _, _ = self._gn_affine(op, op.p[5], op.p[1], op.p[2], op.p[3], N, C)
-        x = self.V(op.p[0], (N, HW, C), (HW * ldx, ldx, 1))
-        v = x.float() * A[:, None] + Bc[:, None]
-        if op.flags & 1:
-            v = F.silu(v)
-        self.V(op.p[4], (N, HW, C), (HW * ldy, ldy, 1)).copy_(v)
+        self.V(op.p[4], (NB, H, W, Cout), (osn, osh, osw, osc)).copy_(y)
 
     def _gn_affine(self, op, stats_ptr, gamma_ptr, beta_ptr, emb_ptr, N, C):
         stats = self.V(stats_ptr, (N, 32, 2), (64, 2, 1))
@@ -265,32 +233,6 @@ class Interp:
     def op_COPY(self, op):
         rows, C, lds, ldd = op.i[:4]
         self.V(op.p[1], (rows, C), (ldd, 1)).copy_(self.V(op.p[0], (rows, C), (lds, 1)).clone())
-
-    def op_TRANSPOSE(self, op):
-        nb1, nb2, R, C = op.i[:4]
-        Rp = op.i[13]
-        for j in range(3):
-            if 2 * j >= len(op.p) or op.p[2 * j] is None:
-                break
-            sb1, sb2, sr = op.i[4 + 3 * j: 7 + 3 * j]
-            src = self.V(op.p[2 * j], (nb1, nb2, R, C), (sb1, sb2, sr, 1))
-            dst = self.V(op.p[2 * j + 1], (nb1, nb2, C, R), (nb2 * C * Rp, C * Rp, Rp, 1))
-            dst.copy_(src.transpose(-1, -2).clone())
-
-    def op_SOFTMAX_FWD(self, op):
-        rows, T, Tp = op.i[:3]
-        S = self.V(op.p[0], (rows, T), (Tp, 1))
-        z = S.float() * op.f[0]
-        if op.p[1] is not None:
-            self.flat(op.p[1], rows).copy_(th.logsumexp(z, dim=-1))
-        S.copy_(th.softmax(z, dim=-1))
-
-    def op_SOFTMAX_BWD(self, op):
-        rows, T, Tp = op.i[:3]
-        P = self.V(op.p[0], (rows, T), (Tp, 1)).float()
-        dPv = self.V(op.p[1], (rows, T), (Tp, 1))
-        dP = dPv.float()
-        dPv.copy_(P * (dP - (P * dP).sum(-1, keepdim=True)) * op.f[0])
 
     def _attn_views(self, op, ptrs):
         B, heads, T, d, qbs, qrs, qhs = op.i[:7]

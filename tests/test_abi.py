@@ -20,12 +20,12 @@ def lib():
     return _lib.load()
 
 
-def test_header_symbols_exported(lib):
+def test_header_symbols_exported_abi_v3(lib):
     declared = set(re.findall(r"^(?:int|const char\*)\s+(cgd_\w+)\s*\(", HEADER, flags=re.M))
     assert declared == set(_lib.EXPORTS), declared ^ set(_lib.EXPORTS)
     for name in declared:
         assert hasattr(lib, name), name
-    assert lib.cgd_abi_version() == 2
+    assert lib.cgd_abi_version() == 3
 
 
 def test_op_tables_match_header():
@@ -44,7 +44,14 @@ def test_plan_create_validates(lib):
     h = ctypes.c_void_p()
     assert lib.cgd_plan_create(bad, 1, ctypes.byref(h)) != 0
     assert b"unknown code" in lib.cgd_last_error()
-    bad[0].code = _lib.OP["CONV"]  # all-zero conv: rejected by argument validation before any CUDA call
+    bad[0].code = 31  # retired (batched-GEMM attention softmax): rejected when the plan is built, not when it runs
+    assert lib.cgd_plan_create(bad, 1, ctypes.byref(h)) != 0
+    assert b"unknown code" in lib.cgd_last_error()
+    bad[0].code = _lib.OP["CONV"]
+    bad[0].i[20] = 8  # reserved operand (was the batched-B mode)
+    assert lib.cgd_plan_create(bad, 1, ctypes.byref(h)) != 0
+    assert b"reserved" in lib.cgd_last_error()
+    bad[0].i[20] = 0  # all-zero conv: rejected by argument validation before any CUDA call
     assert lib.cgd_plan_create(bad, 1, ctypes.byref(h)) != 0
     assert b"conv" in lib.cgd_last_error()
 
@@ -60,7 +67,7 @@ def test_no_cpu_fallback():
         p.run()
 
 
-def test_header_is_plain_c(tmp_path):
+def test_header_is_plain_c_abi_v3(tmp_path):
     """include/cgd_b200.h is the FFI contract: it must compile as C (no C++ or torch types) and link against the built library"""
     import shutil, subprocess
     if shutil.which("gcc") is None:
@@ -75,7 +82,7 @@ def test_header_is_plain_c(tmp_path):
                         "-l:libcgd_b200.so", f"-Wl,-rpath,{libdir}"], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
     out = subprocess.run([str(exe)], capture_output=True, text=True)
-    assert out.returncode == 0 and out.stdout.split() == ["2", str(8 + 24 * 8 + 8 * 4 + 12 * 8)], out.stdout + out.stderr
+    assert out.returncode == 0 and out.stdout.split() == ["3", str(8 + 24 * 8 + 8 * 4 + 12 * 8)], out.stdout + out.stderr
 
 
 def test_product_path_never_imports_the_oracle():

@@ -2,7 +2,7 @@
 Each op is lowered to the C struct with fake, aligned, non-null pointers and handed to `cgd_run_op`: with no device the call must fail
 with a CUDA error (rc > 0: the launch itself), never with rc = -1 (an argument rejected).  Convs stop at the tensor-map encoder
 ("cuTensorMapEncodeTiled unavailable") after their dimension / alignment / stride checks.  This is how op layouts that have not run on
-a device yet (ModifiedResNet tower, epilogue-statistics GroupNorm) are checked against the kernels' contracts."""
+a device yet (ModifiedResNet tower) are checked against the kernels' contracts."""
 import ctypes
 
 import pytest
@@ -49,21 +49,6 @@ def test_resnet_tower_ops_pass_c_side_checks():
             sd[k] += 1
     tower = prn.RNB200(cfg, sd, n_images=4, device="cpu")
     assert _check_plan(tower.plan, "RN tower") > 60
-
-
-def test_epilogue_statistics_ops_pass_c_side_checks():
-    for N, H, W, Cin, C in ((1, 128, 128, 256, 256), (2, 64, 64, 128, 512), (1, 256, 256, 256, 256)):
-        plan = P.Plan()
-        plan.gn_epi_stats, plan.fused_gn, plan.grid_gn = True, False, True
-        cw = P.pack_conv(plan, th.zeros(C, Cin, 3, 3), th.zeros(C), need_bwd=True, name="w")
-        x = plan.act(N, H, W, Cin, "x")
-        h = plan.conv(x, cw, res=plan.act(N, H, W, C, "res"), name="c")
-        y = plan.group_norm(h, plan.const(th.ones(C), "f", "g"), plan.const(th.zeros(C), "f", "b"), emb=(plan.const(th.zeros(N * 2 * C), "f", "e"), 0),
-                            silu=True, name="gn")
-        plan._grads[y.key()] = plan.act(N, H, W, C, "dy")
-        plan.backward()
-        assert P.OP["GN_APPLY_EPI"] in [o.code for o in plan.ops] and plan.ops[0].flags & 2
-        _check_plan(plan, f"epi stats {N}x{H}x{W}")
 
 
 FULL_SIZE = {  # every configuration that runs on the device at full size (tests/test_gpu_baseline_configs.py, test_gpu_fullsize.py, test_gpu_rn.py)

@@ -35,13 +35,13 @@ CASES = [
     ("conv3x3_256x256_c256_dominant_res", 1, 256, 256, 256, 256, 9, True, True),
     ("conv3x3_256x256_c512_to_256", 1, 256, 256, 512, 256, 9, True, False),      # output blocks at 256x256: K = 4608
     ("conv3x3_128x128_c256", 1, 128, 128, 256, 256, 9, True, True),
-    # 8 x 8 images: the weight-streaming kernel (csrc/conv_narrow.cu, conv_small_kernel: 8 output channels per CTA, no split-K) -- the
-    # deepest UNet level's 3x3 convs and attention 1x1s, forward and dgrad, with / without residual, two images
+    # 8 x 8 images: the deepest UNet level's 3x3 convs and attention 1x1s (split-K wgmma tiles), forward and dgrad, with / without
+    # residual, two images
     ("conv3x3_8x8_c1024_res", 1, 8, 8, 1024, 1024, 9, True, True),
     ("conv1x1_8x8_qkv", 1, 8, 8, 1024, 3072, 1, True, False),
     ("conv1x1_8x8_proj_res_b2", 2, 8, 8, 1024, 1024, 1, True, True),
     ("conv1x1_8x8_k3072", 1, 8, 8, 3072, 1024, 1, True, False),
-    ("conv3x3_8x8_c2048_to_1024", 1, 8, 8, 2048, 1024, 9, True, False),   # K too large for the slab: stays on the wgmma split-K path
+    ("conv3x3_8x8_c2048_to_1024", 1, 8, 8, 2048, 1024, 9, True, False),
     # widths of the 128x128 checkpoint (channel_mult 1, 1, 2, 3, 4: a 768-wide 16x16 level, 1280 / 1792-wide concatenations)
     ("conv3x3_16x16_c768_res", 1, 16, 16, 768, 768, 9, True, True),
     ("conv3x3_16x16_c1792_to_768", 1, 16, 16, 1792, 768, 9, True, False),
@@ -201,15 +201,3 @@ def test_narrow_conv_halo_kernel(shape):
     got = plan.view(out, (NB, Cout, H, W))
     err = float((got - ref).abs().max() / ref.abs().max())
     assert th.isfinite(got).all() and err < 2e-3, err
-
-
-def test_small_image_weight_streaming_kernel():
-    """CGD_CONV_SMALL=1: 8 x 8 images take conv_small_kernel (csrc/conv_narrow.cu: a CTA per 8 output channels streaming its whole
-    weight slab, TMA box per activation slice, mma.sync) instead of split-K wgmma tiles.  Opt-in (measured break-even); the switch
-    is read once per process, so the 8 x 8 cases are re-run in a child process with it on."""
-    import os, subprocess, sys
-    env = dict(os.environ, CGD_CONV_SMALL="1")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, "-m", "pytest", "tests/test_gpu_conv.py", "-q", "-x", "-m", "gpu", "-k", "8x8 and (auto or tc2pair) and not small_image",
-                        "-p", "no:cacheprovider"], cwd=root, env=env, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]

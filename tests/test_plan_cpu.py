@@ -153,55 +153,6 @@ def test_cluster_split_picks_are_eligible():
     assert P.pick_cluster_split(2, 1024, 144, 1023) is None  # Cout % 8 != 0: the vector epilogue cannot store it
 
 
-def test_groupnorm_from_conv_epilogue_statistics():
-    """opt-in path (CGD_GN_EPI_STATS / plan.gn_epi_stats): the conv reduces its fp16 output to per-(128-pixel tile, octet) sums
-    (CONV flags 2) and GN_APPLY_EPI normalises in one trip; forward and the backward that consumes its (mean, rstd)."""
-    import torch.nn.functional as F
-    from clip_guided_diffusion_b200 import plan as P
-    from tests.plan_interp import Interp
-    th.manual_seed(0)
-    N, H, W, Cin, C = 2, 32, 32, 64, 256
-    w = th.randn(C, Cin, 3, 3) * (9 * Cin) ** -0.5
-    b = th.randn(C) * 0.1
-    gamma_t, beta_t, emb_t = 1 + 0.1 * th.randn(C), 0.1 * th.randn(C), 0.2 * th.randn(N * 2 * C)
-    outs = {}
-    for epi in (False, True):
-        plan = P.Plan()
-        plan.gn_epi_stats, plan.fused_gn, plan.grid_gn = epi, False, True
-        cw = P.pack_conv(plan, w, b, need_bwd=True, name="w")
-        x = plan.act(N, H, W, Cin, "x")
-        res = plan.act(N, H, W, C, "res")
-        h = plan.conv(x, cw, res=res, name="c")
-        gamma, beta, emb = plan.const(gamma_t, "f", "g"), plan.const(beta_t, "f", "b"), plan.const(emb_t, "f", "e")
-        y = plan.group_norm(h, gamma, beta, emb=(emb, 0), silu=True, name="gn")
-        dy = plan.act(N, H, W, C, "dy")
-        plan._grads[y.key()] = dy
-        plan.mark("bwd")
-        plan.backward()
-        plan.finalize("cpu")
-        codes = [o.code for o in plan.ops]
-        assert (P.OP["GN_APPLY_EPI"] in codes) == epi and (P.OP["GN_FWD_GRID"] in codes) == (not epi)
-        conv_op = plan.ops[0]
-        assert bool(conv_op.flags & 2) == epi
-        g = th.Generator().manual_seed(1)
-        plan.view(x.buf, (N, H, W, Cin)).copy_(th.randn(N, H, W, Cin, generator=g))
-        plan.view(res.buf, (N, H, W, C)).copy_(th.randn(N, H, W, C, generator=g))
-        plan.view(dy.buf, (N, H, W, C)).copy_(th.randn(N, H, W, C, generator=g))
-        Interp(plan).run()
-        outs[epi] = (plan.view(y.buf, (N, H, W, C)).float().clone(), plan.view(plan.grad_of(x).buf, (N, H, W, Cin)).float().clone(),
-                     plan.view(h.buf, (N, H, W, C)).float().clone())
-    y0, dx0, h0 = outs[False]
-    y1, dx1, h1 = outs[True]
-    assert th.equal(h0, h1)
-    assert float((y1 - y0).abs().max()) < 4e-3 * float(y0.abs().max())  # same statistics up to summation order, fp16 outputs
-    assert float((dx1 - dx0).norm() / dx0.norm()) < 2e-3
-    # and against torch directly: GroupNorm of the stored fp16 conv output, scale-shift, SiLU
-    e = emb_t.view(N, 2 * C)
-    ref = F.group_norm(h1.permute(0, 3, 1, 2), 32, gamma_t, beta_t, eps=1e-5) * (1 + e[:, :C, None, None]) + e[:, C:, None, None]
-    ref = F.silu(ref).permute(0, 2, 3, 1)
-    assert float((y1 - ref).abs().max()) < 4e-3 * float(ref.abs().max())
-
-
 def test_engine_model_load_state_dict_repacks_in_place():
     """cgd/script_util.py:317: `model.load_state_dict(checkpoint)` on the engine's UNet handle re-packs the checkpoint into the
     kernel layouts in place: the arena must equal, byte for byte, the arena of an engine CONSTRUCTED from that checkpoint."""
