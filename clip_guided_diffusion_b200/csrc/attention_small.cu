@@ -3,7 +3,7 @@
 //
 // Replaces [3P] CLIP nn.MultiheadAttention's core for ViT-B/32 (50 tokens) and [3P] guided-diffusion QKVAttention(Legacy) at the
 // 8x8 UNet level (64 tokens) (SURVEY.md K4, K14).  Why a separate kernel: these problems are one 64x64 tile per head -- the
-// flash kernels of attention_mma.cu need two launches for the backward.  Here the
+// flash kernels of attention_flash.cu need two launches for the backward.  Here the
 // whole backward -- S, P, dP, dS, dQ, dK, dV -- is one launch; P and dS go through shared memory once (fp16, like the
 // reference's fp16 attention weights) to feed the transposed products.
 #include <cuda_fp16.h>
@@ -15,18 +15,8 @@
 
 namespace cgd {
 
-struct AttnSmallArgs {
-  const __half *q, *k, *v, *dout;
-  __half *out, *dq, *dk, *dv;
-  float* lse;
-  int B, heads, T;
-  int64_t qbs, qrs, qhs;  // qkv batch / row / head strides (elements)
-  int64_t obs, ors, ohs;  // out / dout strides
-  float scale;
-};
-
-__global__ void __launch_bounds__(128) attn_small_fwd_kernel(const AttnSmallArgs a) {
-  __shared__ __align__(16) __half Qs[AS_T * AS_LD], Ks[AS_T * AS_LD], Vs[AS_T * AS_LD];
+__global__ void __launch_bounds__(128) attn_small_fwd_kernel(const AttnArgs a) {
+  __shared__ __align__(16) __half Qs[AS_TILE], Ks[AS_TILE], Vs[AS_TILE];
   pdl_wait();
   pdl_launch_dependents();
   const int h = blockIdx.x, b = blockIdx.y;
@@ -54,9 +44,9 @@ __global__ void __launch_bounds__(128) attn_small_fwd_kernel(const AttnSmallArgs
   as_store_c(o, a.out + (int64_t)b * a.obs + (int64_t)h * a.ohs, a.ors, r0, a.T, lane);
 }
 
-__global__ void __launch_bounds__(128) attn_small_bwd_kernel(const AttnSmallArgs a) {
+__global__ void __launch_bounds__(128) attn_small_bwd_kernel(const AttnArgs a) {
   extern __shared__ __align__(16) __half as_dyn[];
-  __half *Qs = as_dyn, *Ks = Qs + AS_T * AS_LD, *Vs = Ks + AS_T * AS_LD, *dOs = Vs + AS_T * AS_LD, *Ps = dOs + AS_T * AS_LD, *dSs = Ps + AS_T * AS_LD;
+  __half *Qs = as_dyn, *Ks = Qs + AS_TILE, *Vs = Ks + AS_TILE, *dOs = Vs + AS_TILE, *Ps = dOs + AS_TILE, *dSs = Ps + AS_TILE;
   pdl_wait();
   pdl_launch_dependents();
   const int h = blockIdx.x, b = blockIdx.y;
@@ -92,15 +82,7 @@ __global__ void __launch_bounds__(128) attn_small_bwd_kernel(const AttnSmallArgs
       dp[j][2] = s[j][2] * (dp[j][2] - d1) * a.scale;
       dp[j][3] = s[j][3] * (dp[j][3] - d1) * a.scale;
     }
-    // P and dS to shared memory (fp16, [q][key]) for the transposed products
-    const int ra = r0 + (lane >> 2), cb = (lane & 3) * 2;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      *reinterpret_cast<__half2*>(Ps + ra * AS_LD + j * 8 + cb) = __floats2half2_rn(s[j][0], s[j][1]);
-      *reinterpret_cast<__half2*>(Ps + (ra + 8) * AS_LD + j * 8 + cb) = __floats2half2_rn(s[j][2], s[j][3]);
-      *reinterpret_cast<__half2*>(dSs + ra * AS_LD + j * 8 + cb) = __floats2half2_rn(dp[j][0], dp[j][1]);
-      *reinterpret_cast<__half2*>(dSs + (ra + 8) * AS_LD + j * 8 + cb) = __floats2half2_rn(dp[j][2], dp[j][3]);
-    }
+    as_store_p_ds(s, dp, Ps, dSs, r0, lane);
     uint32_t dsa[4][4];
     as_c_to_a(dp, dsa);
     float dq[8][4];
@@ -120,31 +102,12 @@ __global__ void __launch_bounds__(128) attn_small_bwd_kernel(const AttnSmallArgs
 
 int attn_small_supported(int64_t T) { return T >= 1 && T <= AS_T; }
 
-static int attn_small_args(const CgdOp& op, AttnSmallArgs& a, bool bwd) {
-  a.B = (int)op.i[0]; a.heads = (int)op.i[1]; a.T = (int)op.i[2];
-  a.qbs = op.i[4]; a.qrs = op.i[5]; a.qhs = op.i[6]; a.obs = op.i[7]; a.ors = op.i[8]; a.ohs = op.i[9];
-  a.scale = op.f[0];
-  a.q = (const __half*)op.p[0]; a.k = (const __half*)op.p[1]; a.v = (const __half*)op.p[2];
-  if (!bwd) {
-    a.out = (__half*)op.p[3];
-    a.lse = (float*)op.p[4];
-  } else {
-    a.dout = (const __half*)op.p[4];
-    a.dq = (__half*)op.p[6]; a.dk = (__half*)op.p[7]; a.dv = (__half*)op.p[8];
-  }
-  return 0;
-}
-
-int launch_attn_small_fwd(const CgdOp& op, cudaStream_t st) {
-  AttnSmallArgs a{};
-  attn_small_args(op, a, false);
+int launch_attn_small_fwd(const AttnArgs& a, cudaStream_t st) {
   CGD_CUDA(launch_pdl(attn_small_fwd_kernel, dim3(a.heads, a.B), dim3(128), 0, st, a));
   return 0;
 }
-int launch_attn_small_bwd(const CgdOp& op, cudaStream_t st) {
-  AttnSmallArgs a{};
-  attn_small_args(op, a, true);
-  constexpr int smem = 6 * AS_T * AS_LD * (int)sizeof(__half);
+int launch_attn_small_bwd(const AttnArgs& a, cudaStream_t st) {
+  constexpr int smem = 6 * AS_TILE * (int)sizeof(__half);
   static DeviceOnce set;
   if (set.needed()) {
     CGD_CUDA(cudaFuncSetAttribute(attn_small_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));

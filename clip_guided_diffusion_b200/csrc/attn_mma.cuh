@@ -1,5 +1,5 @@
 // attn_mma.cuh -- warp-level tensor-core building blocks (mma.sync m16n8k16, ldmatrix) shared by the single-tile attention
-// (attention_small.cu) and the flash attention kernels (attention_mma.cu): 64 x 64 fp16 tiles in shared memory, row pitch 72.
+// (attention_small.cu) and the flash attention kernels (attention_flash.cu): 64 x 64 fp16 tiles in shared memory, row pitch 72.
 #pragma once
 #include <cuda_fp16.h>
 
@@ -9,7 +9,18 @@ namespace cgd {
 
 constexpr int AS_T = 64;        // tile edge: queries, keys, head dim
 constexpr int AS_LD = AS_T + 8; // shared-memory row pitch in halfs (144 B: 16-byte aligned, ldmatrix conflict-free)
+constexpr int AS_TILE = AS_T * AS_LD;  // halfs per shared tile
 
+// Operands of one ATTN_FWD / ATTN_BWD op (slots in include/cgd_b200.h), unpacked once by attention.cu
+struct AttnArgs {
+  const __half *q, *k, *v, *o, *dout;
+  __half *out, *dq, *dk, *dv;
+  float *lse, *delta;
+  int B, heads, T;
+  int64_t qbs, qrs, qhs;  // qkv batch / row / head strides (elements)
+  int64_t obs, ors, ohs;  // out / dout strides
+  float scale;
+};
 
 __device__ __forceinline__ uint32_t as_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
@@ -181,6 +192,16 @@ __device__ __forceinline__ void as_store_c(const float (&c)[8][4], __half* g, in
     if (rb < T) *reinterpret_cast<__half2*>(g + (int64_t)rb * rs + j * 8 + cb) = __floats2half2_rn(c[j][2], c[j][3]);
   }
 }
-
+// P and dS fragments of rows r0 + lane/4 (+8) -> fp16 shared tiles ([query][key]) for the transposed products dV = P^T dO, dK = dS^T Q
+__device__ __forceinline__ void as_store_p_ds(const float (&p)[8][4], const float (&ds)[8][4], __half* Ps, __half* dSs, int r0, int lane) {
+  const int ra = r0 + (lane >> 2), cb = (lane & 3) * 2;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    *reinterpret_cast<__half2*>(Ps + ra * AS_LD + j * 8 + cb) = __floats2half2_rn(p[j][0], p[j][1]);
+    *reinterpret_cast<__half2*>(Ps + (ra + 8) * AS_LD + j * 8 + cb) = __floats2half2_rn(p[j][2], p[j][3]);
+    *reinterpret_cast<__half2*>(dSs + ra * AS_LD + j * 8 + cb) = __floats2half2_rn(ds[j][0], ds[j][1]);
+    *reinterpret_cast<__half2*>(dSs + (ra + 8) * AS_LD + j * 8 + cb) = __floats2half2_rn(ds[j][2], ds[j][3]);
+  }
+}
 
 }  // namespace cgd

@@ -1,6 +1,6 @@
-"""GPU: softmax attention (head dim 64; 128 / 192 / 256 for the 128x128 checkpoint's four heads: csrc/attention_wide.cu) forward and
-input-gradient -- the single-tile tensor-core kernels (T <= 64: csrc/attention_small.cu) and the flash kernels (csrc/attention_mma.cu)
--- against a plain PyTorch fp32 reference of [3P] QKVAttentionLegacy / QKVAttention / nn.MultiheadAttention's core (SURVEY.md K4, K14)."""
+"""GPU: softmax attention (head dim 64; 128 / 192 / 256 for the 128x128 checkpoint's four heads) forward and input-gradient -- the
+single-tile tensor-core kernels (head dim 64, T <= 64: csrc/attention_small.cu) and the flash kernels (every other case:
+csrc/attention_flash.cu) -- against a plain PyTorch fp32 reference of [3P] QKVAttentionLegacy / QKVAttention / nn.MultiheadAttention's core (SURVEY.md K4, K14)."""
 import math
 
 import pytest

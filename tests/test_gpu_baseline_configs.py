@@ -31,7 +31,7 @@ CASES = {
     "cfg4": dict(size=512, respacing="ddim250", cutn=16, clip="ViT-B/16", lpips=False, t_index=120),
     "cfg5": dict(size=512, respacing="1000", cutn=64, clip="ViT-L/14", lpips=True, t_index=400),
     # not a BASELINE configuration: the reference's DEFAULT call (cgd/cgd.py:20-33: image_size 128, "1000", 16 cutouts, ViT-B/32) -- the
-    # 128x128 checkpoint, whose four heads attend with 128 / 192 / 256 channels each (csrc/attention_wide.cu)
+    # 128x128 checkpoint, whose four heads attend with 128 / 192 / 256 channels each (csrc/attention_flash.cu)
     "default128": dict(size=128, respacing="1000", cutn=16, clip="ViT-B/32", lpips=False, t_index=500),
     # the one CLIP_MODEL_URLS entry (cgd/clip_util.py:28) whose cutouts are not 224 px: 336 px, 24 x 24 patches of 14, 577 tokens
     "vit_l14_336": dict(size=256, respacing="ddim250", cutn=4, clip="ViT-L/14@336px", lpips=False, t_index=180),

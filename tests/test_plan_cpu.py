@@ -57,7 +57,7 @@ def test_unet_plan_matches_oracle(new_order, cond):
 @pytest.mark.parametrize("heads,mult", [(1, (1, 2)), (1, (1, 2, 3))])
 def test_unet_plan_with_num_heads_wide_head_dims(heads, mult):
     """the 128x128 checkpoint's attention (data/diffusion_model_flags.py: num_heads = 4, num_head_channels unset -> head dim =
-    channels / num_heads = 128 / 192 / 256; csrc/attention_wide.cu): here 128 and 192 channels in one head, legacy qkv order"""
+    channels / num_heads = 128 / 192 / 256; csrc/attention_flash.cu): here 128 and 192 channels in one head, legacy qkv order"""
     import dataclasses
     th.manual_seed(0)
     size = 16 * 2 ** (len(mult) - 1)
