@@ -2,14 +2,19 @@
 
 Same keyword arguments and the same generator contract (yields ``(batch_idx, png_path)``); set-up stays Python and
 runs once (seed, prompt encoding, weight loading, cutout cache), the per-timestep work is the engine's fused step.
-Out of scope here, exactly as SURVEY.md section 2 marks them: checkpoint download, W&B, GIF/MP4,
-image prompts (the reference's ``encode_image_prompt`` crashes, quirk B5).  The LPIPS init loss (``init_image`` + ``init_scale``)
-runs on the engine when the VGG weights are given (``lpips_state_dict=``) or the ``lpips`` package is installed.
+Out of scope here, exactly as SURVEY.md section 2 marks them: checkpoint download, W&B, GIF/MP4.  The LPIPS init loss
+(``init_image`` + ``init_scale``) runs on the engine when the VGG weights are given (``lpips_state_dict=``) or the ``lpips`` package
+is installed.
+
+Image prompts (``image_prompts=["path:weight", ...]``, local files) are encoded once, before the loop, by ``encode_image_prompt``:
+the intent of the reference's function of that name, which itself crashes (quirk B5; image_prompt.py).  Each one adds
+``num_cutouts`` target embeddings of weight ``weight / num_cutouts`` after the text prompts' embeddings; the weights of the whole set
+are then normalised together (cgd/cgd.py:86-105).
 
 Weights: pass ``unet_state_dict`` / ``clip_state_dict`` (upstream key layout), or have the reference's checkpoints on
 disk under ``checkpoints_dir`` (``256x256_diffusion.pt`` ..., ``clip/ViT-B-32.pt``).  Text prompts need a text tower:
 either pass ``target_embeds`` / ``weights`` directly or have the ``clip`` package importable (used once, outside the hot
-path, like cgd/clip_util.py:104-108).
+path, like cgd/clip_util.py:104-108).  Image prompts use this package's own CLIP visual tower and never import ``clip``.
 """
 from __future__ import annotations
 
@@ -20,6 +25,7 @@ import torch as th
 
 from . import gaussian_diffusion as gd
 from .guidance import CondFnB200, GuidedStepB200, MakeCutouts
+from .image_prompt import ImagePromptEncoder, check_local
 from .unet import config_for
 from .rn import RN_CONFIGS, rn_config_from_state_dict
 from .vit import VIT_CONFIGS, vit_config_from_state_dict
@@ -135,6 +141,26 @@ def _tower_config(clip_sd: dict):
     return vit_config_from_state_dict(clip_sd)
 
 
+def _clip_tower(clip_model_name, clip_state_dict, checkpoints_dir):
+    """-> (CLIP state_dict, visual tower config): the given state_dict's own architecture, or the named tower's checkpoint"""
+    clip_sd = clip_state_dict if clip_state_dict is not None else _load_clip_sd(clip_model_name, checkpoints_dir)
+    towers = {**VIT_CONFIGS, **RN_CONFIGS}
+    if clip_state_dict is None and clip_model_name not in towers:
+        raise NotImplementedError(f"CLIP tower {clip_model_name!r} is not supported (supported: {sorted(towers)})")
+    return clip_sd, (_tower_config(clip_sd) if clip_state_dict is not None else towers[clip_model_name])
+
+
+def encode_image_prompt(image: str, weight: float, diffusion_size: int, num_cutouts: int, clip_model_name: str = "ViT-B/32",
+                        device: str = "cuda", *, clip_state_dict: dict = None, checkpoints_dir: str = CACHE_PATH):
+    """cgd/clip_util.py:90-101 (the reference's signature plus the weight source) -> (embeds fp32 [num_cutouts, D] on ``device``,
+    ``[weight / num_cutouts] * num_cutouts``).  ``image`` is a local file; the cutout windows are drawn from the CPU default
+    generator.  For callers that assemble ``target_embeds=`` / ``weights=`` themselves: append the result after the text prompts'
+    embeddings, as ``clip_guided_diffusion(image_prompts=...)`` does."""
+    _require_cuda(device)
+    clip_sd, cfg = _clip_tower(clip_model_name, clip_state_dict, checkpoints_dir)
+    return ImagePromptEncoder(cfg, clip_sd, num_cutouts, device).encode(image, weight, diffusion_size)
+
+
 def _require_cuda(device):
     if not str(device).startswith("cuda") or not th.cuda.is_available():
         raise RuntimeError("clip_guided_diffusion_b200 runs the sampling step on a CUDA (sm_90a, H100) device only; there is no CPU path")
@@ -157,8 +183,12 @@ def clip_guided_diffusion(
     if len(device) == 0:
         device = "cuda"
     _require_cuda(device)
-    if image_prompts:
-        raise NotImplementedError("image prompts are unsupported (the reference's encode_image_prompt crashes, SURVEY quirk B5)")
+    if image_prompts and target_embeds is not None:
+        raise NotImplementedError("target_embeds= is the complete target set: with image prompts, encode them with encode_image_prompt() "
+                                  "and append the embeddings and weights to target_embeds= / weights= instead of passing image_prompts=")
+    image_prompts = [parse_prompt(p) for p in image_prompts]  # "path:weight" (cgd/cgd.py:93)
+    for path, _ in image_prompts:
+        check_local(path)
     if wandb_project is not None:
         raise NotImplementedError("W&B logging is outside the hot path (SURVEY section 2)")
     th.manual_seed(seed)
@@ -166,13 +196,24 @@ def clip_guided_diffusion(
         use_magnitude = True
     Path(prefix_path).mkdir(parents=True, exist_ok=True)
 
-    clip_sd = clip_state_dict if clip_state_dict is not None else _load_clip_sd(clip_model_name, checkpoints_dir)
-    towers = {**VIT_CONFIGS, **RN_CONFIGS}
-    if clip_state_dict is None and clip_model_name not in towers:
-        raise NotImplementedError(f"CLIP tower {clip_model_name!r} is not supported (supported: {sorted(towers)})")
-    vit_cfg = _tower_config(clip_sd) if clip_state_dict is not None else towers[clip_model_name]
+    clip_sd, vit_cfg = _clip_tower(clip_model_name, clip_state_dict, checkpoints_dir)
     if target_embeds is None:
-        target_embeds, weights = _encode_text(prompts, clip_model_name, device)
+        # text prompts first, then every image prompt's cutn embeddings (cgd/cgd.py:86-98); an image-only run needs no text tower
+        embeds, weights = [], []
+        if prompts or not image_prompts:
+            e, w = _encode_text(prompts, clip_model_name, device)
+            embeds.append(e)
+            weights += [float(v) for v in w]
+        if image_prompts:
+            # one forward-only tower for every image prompt, released before the engine is built; its cutout windows come from the
+            # CPU generator after the seed and before cache_coordinates / the loop, where the reference draws them
+            encoder = ImagePromptEncoder(vit_cfg, clip_sd, num_cutouts, device)
+            for path, w in image_prompts:
+                e, ws = encoder.encode(path, w, image_size)
+                embeds.append(e)
+                weights += ws
+            del encoder
+        target_embeds, weights = th.cat([e.to(device) for e in embeds]), th.tensor(weights)
     if weights is None:  # target_embeds= given without weights=: every prompt weighs 1 (parse_prompt's default)
         weights = th.ones(target_embeds.shape[0])
     weights = th.as_tensor(weights, dtype=th.float32)

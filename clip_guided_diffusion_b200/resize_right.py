@@ -1,4 +1,5 @@
-"""Host side of the ResizeRight cutout mode: per-(crop size, output size) 1-D resampling tables for the CUDA cutout kernels.
+"""Host side of the ResizeRight resampler: per-(input size, output size) 1-D resampling tables for the CUDA cutout kernels (at most
+``T_MAX`` taps) and for the ``RESIZE_AXIS`` op of image prompts (``t_max=None``: any tap count).
 
 ``north_star`` names "MakeCutouts' random-crop + ResizeRight downsample"; the reference's MakeCutouts actually pools
 (cgd/modules.py:63) and only ``encode_image_prompt`` calls the vendored resampler (cgd/clip_util.py:95-97, lanczos3, antialiasing).
@@ -30,13 +31,14 @@ def _lanczos3(x: th.Tensor) -> th.Tensor:  # cgd/ResizeRight/interp_methods.py:5
     return ((th.sin(pi * x) * th.sin(pi * x / 3) + _EPS) / ((pi ** 2 * x ** 2 / 3) + _EPS)) * (abs(x) < 3).to(x.dtype)
 
 
-def tables(S: int, O: int):
-    """-> (left int32 [O] relative to the crop, weights float32 [O, T_MAX] zero-padded, taps T)"""
-    key = (int(S), int(O))
+def tables(S: int, O: int, t_max: "int | None" = T_MAX):
+    """-> (left int32 [O] relative to the crop, weights float32 [O, t_max] zero-padded, taps T).
+    ``t_max=None``: no cap, the weights are [O, T] (the RESIZE_AXIS op of image prompts, any scale factor)."""
+    key = (int(S), int(O), t_max)
     if key in _cache:
         return _cache[key]
     if S == O:  # scale factor 1: the reference leaves the dimension untouched (resize_right.py:58-62)
-        wt = th.zeros(O, T_MAX)
+        wt = th.zeros(O, t_max or 1)
         wt[:, 0] = 1.0
         res = (th.arange(O, dtype=th.int32), wt, 1)
         _cache[key] = res
@@ -52,15 +54,15 @@ def tables(S: int, O: int):
         kern = _lanczos3
     left = (grid - support / 2 - _EPS).ceil().long()
     T = ceil(support - _EPS)
-    if T > T_MAX:
-        raise ValueError(f"resize {S} -> {O}: {T} taps exceed the device tables ({T_MAX}); scale factors below 0.4 are unsupported")
+    if t_max is not None and T > t_max:
+        raise ValueError(f"resize {S} -> {O}: {T} taps exceed the device tables ({t_max}); scale factors below 0.4 are unsupported")
     fov = left[:, None] + th.arange(T)
     pad = -int(fov[0, 0])  # the reference shifts grid and field of view by the left padding before evaluating the kernel
     w = kern((grid + pad)[:, None] - (fov + pad))
     sw = w.sum(1, keepdim=True)
     sw[sw == 0] = 1
     w = w / sw
-    wt = th.zeros(O, T_MAX)
+    wt = th.zeros(O, t_max or T)
     wt[:, :T] = w
     res = (left.to(th.int32).contiguous(), wt.contiguous(), T)
     _cache[key] = res

@@ -227,6 +227,11 @@ enum {
    * _BWD: the transposed gather scattered with fp32 atomics INTO p2 dx (zero it first: CGD_OP_FILL); p3 params; f6 gradient scale */
   CGD_OP_CUTOUTS_AUG_FWD = 50,
   CGD_OP_CUTOUTS_AUG_BWD = 51,
+  /* one axis of a separable resampling (image prompts: ResizeRight lanczos3 with antialiasing, cgd/clip_util.py:95-97), with host-built
+   * tables of any tap count: out[.., o, ..] = sum_{i<T} w[o,i] * in[.., left[o] + i, ..], samples outside [0, S) are zero; fp32, summed
+   * in tap order.  p0 in(f [planes, H, W]) p1 out(f [planes, O, W] for axis 0, [planes, H, O] for axis 1) p2 left(i32 [O])
+   * p3 weights(f [O, T]) ; i0 planes i1 H i2 W i3 axis (0 = H, 1 = W) i4 O i5 T */
+  CGD_OP_RESIZE_AXIS = 52,
   CGD_OP__COUNT
 };
 
