@@ -14,7 +14,8 @@
 // registers.  Pipeline: STAGES-deep smem ring with full/empty mbarriers; a stage is released once
 // the wgmma group that read it has retired (wait_group 1 keeps one group in flight).
 // Epilogue: the accumulators go to an fp32 staging tile that reuses the ring; then each consumer thread
-// owns one pixel row and half of the tile's channels and adds bias / residual, stores fp16 / fp32.
+// owns one pixel row and half of the tile's channels and adds bias / residual, stores fp16 / fp32 (split-K:
+// one 8-channel chunk of a row per pass, neighbouring threads on neighbouring chunks).
 // Small-M layers (8x8 .. 32x32 feature maps, long-K Linears) split K over gridDim.z: either into an
 // fp32 workspace summed by a reduce kernel, or (CONV i23 = 1) inside a thread-block cluster of
 // `splits` CTAs that sum each other's staging tiles through distributed shared memory -- one launch,
@@ -156,45 +157,47 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (p.cluster) cluster_sync_all();  // every CTA of the cluster has staged its partial tile
 
   if (warp < kConsumers / 32) {
-    // ===== epilogue: thread = (pixel row r, half of the columns this CTA finishes)
-    const int quad = warp & 3, half = warp >> 2;
-    const int r = quad * 32 + lane;
-    const int w_off = r % p.TW, h_off = (r / p.TW) % p.TH, n_off = r / (p.TW * p.TH);
-    const int n = n0 + n_off, h = h0 + h_off, w = w0 + w_off;
-    const bool row_ok = (n < p.NB) && (h < p.H) && (w < p.W);
+    // ===== epilogue: 8 consecutive columns c of pixel row r at a time
     const int S = p.cluster ? p.splits : 1;
     const int cw = BN / S;  // columns finished by this CTA (a multiple of 16: host)
-    const int c_lo = (p.cluster ? (int)cluster_ctarank() * cw : 0) + half * (cw / 2), c_hi = c_lo + cw / 2;
-    const float* srow = staging + (size_t)r * Cfg::kStageLd;
-    const int64_t o_off = (int64_t)n * p.out_sn + (int64_t)h * p.out_sh + (int64_t)w * p.out_sw;
-    const int64_t r_off = (int64_t)n * p.res_sn + (int64_t)h * p.res_sh + (int64_t)w * p.res_sw;
+    const int c_base = p.cluster ? (int)cluster_ctarank() * cw : 0;
     const bool vec_ok = !p.out_f32 && p.out_sc == 1;
     const bool to_ws = p.splits > 1 && !p.cluster;
-    float* ws = to_ws ? p.ws + ((size_t)blockIdx.z * p.ws_rows + (size_t)mt * BM + r) * p.Npad + ncol0 : nullptr;
-#pragma unroll 1
-    for (int c = c_lo; c < c_hi; c += 8) {
+    auto finish8 = [&](const int r, const int c) {
+      const int w_off = r % p.TW, h_off = (r / p.TW) % p.TH, n_off = r / (p.TW * p.TH);
+      const int n = n0 + n_off, h = h0 + h_off, w = w0 + w_off;
+      const bool row_ok = (n < p.NB) && (h < p.H) && (w < p.W);
+      const float* srow = staging + (size_t)r * Cfg::kStageLd;
+      const int64_t o_off = (int64_t)n * p.out_sn + (int64_t)h * p.out_sh + (int64_t)w * p.out_sw;
+      const int64_t r_off = (int64_t)n * p.res_sn + (int64_t)h * p.res_sh + (int64_t)w * p.res_sw;
       float a[8];
+      // chunks with bit 5 of c set read their upper 4 columns first: with 8-column chunks side by side in a warp, the two float4
+      // reads then spread over all 8 16-byte bank groups (4 wavefronts each instead of 8)
+      const bool swap = (c & 32) != 0;
       if (p.cluster) {  // fixed order over the cluster's partial tiles: bit-reproducible
 #pragma unroll
         for (int e = 0; e < 8; ++e) a[e] = 0.f;
         const uint32_t local = smem_u32(srow + c);
         for (int j = 0; j < S; ++j) {
           const uint32_t remote = mapa_u32(local, (uint32_t)j);
-          const float4 u0 = ld_cluster_f4(remote), u1 = ld_cluster_f4(remote + 16);
+          float4 u0 = ld_cluster_f4(remote + (swap ? 16 : 0)), u1 = ld_cluster_f4(remote + (swap ? 0 : 16));
+          if (swap) { const float4 tmp = u0; u0 = u1; u1 = tmp; }
           a[0] += u0.x; a[1] += u0.y; a[2] += u0.z; a[3] += u0.w;
           a[4] += u1.x; a[5] += u1.y; a[6] += u1.z; a[7] += u1.w;
         }
       } else {
-        const float4 u0 = *reinterpret_cast<const float4*>(srow + c), u1 = *reinterpret_cast<const float4*>(srow + c + 4);
+        float4 u0 = *reinterpret_cast<const float4*>(srow + c + (swap ? 4 : 0)), u1 = *reinterpret_cast<const float4*>(srow + c + (swap ? 0 : 4));
+        if (swap) { const float4 tmp = u0; u0 = u1; u1 = tmp; }
         a[0] = u0.x; a[1] = u0.y; a[2] = u0.z; a[3] = u0.w;
         a[4] = u1.x; a[5] = u1.y; a[6] = u1.z; a[7] = u1.w;
       }
       if (to_ws) {  // raw fp32 partials -> workspace [split][tile row][Npad]; rows outside the image are never read back
         if (row_ok) {
+          float* ws = p.ws + ((size_t)blockIdx.z * p.ws_rows + (size_t)mt * BM + r) * p.Npad + ncol0;
           *reinterpret_cast<float4*>(ws + c) = make_float4(a[0], a[1], a[2], a[3]);
           *reinterpret_cast<float4*>(ws + c + 4) = make_float4(a[4], a[5], a[6], a[7]);
         }
-        continue;
+        return;
       }
       const int col = ncol0 + c;
       if (row_ok && col < p.Cout) {
@@ -230,6 +233,27 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           }
         }
       }
+    };
+    if (p.cluster || to_ws) {
+      // split-K: consecutive threads take consecutive 8-column chunks of one row, so a warp's fp32 partial stores to the workspace
+      // (or its distributed-shared-memory reads of the cluster's staging rows) cover contiguous runs of a row; with one pixel row
+      // per thread every 32-byte partial store of a warp lands on 32 rows (on an H100 the workspace split-K 3x3 convs of the
+      // 32 x 32 and 16 x 16 levels took 1.4-1.5x as long)
+      const int cpr = cw / 8;              // chunks per row
+      const int rows_per_pass = kConsumers / cpr;
+      const int t = threadIdx.x;
+      if (t < rows_per_pass * cpr) {
+        const int c = c_base + (t % cpr) * 8;
+#pragma unroll 1
+        for (int r = t / cpr; r < BM; r += rows_per_pass) finish8(r, c);
+      }
+    } else {
+      // thread = (pixel row r, half of the columns): measured faster than the chunk mapping above on the one-CTA 256 x 256 layers,
+      // and the coalesced order for channel-strided (NCHW fp32) outputs
+      const int r = (warp & 3) * 32 + lane, half = warp >> 2;
+      const int c_lo = c_base + half * (cw / 2), c_hi = c_lo + cw / 2;
+#pragma unroll 1
+      for (int c = c_lo; c < c_hi; c += 8) finish8(r, c);
     }
   }
   if (p.cluster) cluster_sync_all();  // the other CTAs' reads of this CTA's staging tile are complete before it exits
