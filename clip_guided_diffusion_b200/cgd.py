@@ -12,9 +12,15 @@ the intent of the reference's function of that name, which itself crashes (quirk
 are then normalised together (cgd/cgd.py:86-105).
 
 Weights: pass ``unet_state_dict`` / ``clip_state_dict`` (upstream key layout), or have the reference's checkpoints on
-disk under ``checkpoints_dir`` (``256x256_diffusion.pt`` ..., ``clip/ViT-B-32.pt``).  Text prompts need a text tower:
-either pass ``target_embeds`` / ``weights`` directly or have the ``clip`` package importable (used once, outside the hot
-path, like cgd/clip_util.py:104-108).  Image prompts use this package's own CLIP visual tower and never import ``clip``.
+disk under ``checkpoints_dir`` (``256x256_diffusion.pt`` ..., ``clip/ViT-B-32.pt``).  Text prompts are encoded once, outside the hot
+path (cgd/clip_util.py:104-108), by one of two text towers (``text_encoder=``):
+- ``"device"``: this package's own tokenizer and causal text tower (tokenizer.py, text.py), from the same CLIP state_dict as the
+  visual tower; needs CLIP's BPE vocabulary file (``bpe_path=``, or ``bpe_simple_vocab_16e6.txt.gz`` under ``checkpoints_dir/clip/``
+  or ``CACHE_PATH/clip/``);
+- ``"clip"``: the ``clip`` package's eager model (``clip.load(clip_model_name)``, its own checkpoint);
+- ``"auto"`` (default): the ``clip`` package if it imports, else the device tower if the vocabulary file is found, else the ``clip``
+  path, which raises without the package.
+Or pass ``target_embeds`` / ``weights`` directly.  Image prompts use this package's own CLIP visual tower and never import ``clip``.
 """
 from __future__ import annotations
 
@@ -26,6 +32,8 @@ import torch as th
 from . import gaussian_diffusion as gd
 from .guidance import CondFnB200, GuidedStepB200, MakeCutouts
 from .image_prompt import ImagePromptEncoder, check_local
+from .text import TextB200, text_config_from_state_dict
+from .tokenizer import find_vocab, load_tokenizer, tokenize  # noqa: F401 (tokenize: public, like clip.tokenize)
 from .unet import config_for
 from .rn import RN_CONFIGS, rn_config_from_state_dict
 from .vit import VIT_CONFIGS, vit_config_from_state_dict
@@ -118,6 +126,49 @@ def _encode_text(prompts, clip_model_name, device):
     return th.cat(embeds), th.tensor(weights)
 
 
+def _clip_importable() -> bool:
+    """does `import clip` succeed?  (a package that is installed but fails to import counts as absent)"""
+    try:
+        import clip  # noqa: F401
+    except Exception:  # noqa: BLE001 -- any import failure means the clip path cannot run
+        return False
+    return True
+
+
+def _text_encoder_choice(text_encoder, bpe_path, checkpoints_dir):
+    """-> the vocabulary file when the device tower encodes the text prompts, None when `_encode_text` (the `clip` package) does"""
+    if text_encoder == "clip" or (text_encoder == "auto" and _clip_importable()):
+        return None
+    try:
+        return find_vocab(bpe_path, checkpoints_dir)
+    except FileNotFoundError:
+        if text_encoder == "device":
+            raise
+        return None
+
+
+def _encode_text_device(prompts, clip_sd, vocab, device):
+    """all text prompts in one pass of a forward-only text tower, in prompt order -> (fp32 [P, D], weights [P])"""
+    parsed = [parse_prompt(p) for p in prompts]
+    cfg = text_config_from_state_dict(clip_sd)
+    ids = load_tokenizer(vocab).tokenize([t for t, _ in parsed], context_length=cfg.context_length)
+    tower = TextB200(cfg, clip_sd, len(parsed), device)
+    embeds = tower.encode(ids)
+    del tower
+    return embeds, th.tensor([w for _, w in parsed])
+
+
+def encode_text_prompt(txt: str, weight: float, clip_model_name: str = "ViT-B/32", device: str = "cuda", *, clip_state_dict: dict = None,
+                       checkpoints_dir: str = CACHE_PATH, bpe_path: str = None):
+    """cgd/clip_util.py:104-108 (the reference's signature plus the weight and vocabulary sources) -> (fp32 [1, D] on ``device``,
+    ``weight``), on this package's text tower: the text half of ``clip_state_dict`` or of the named checkpoint, and the BPE vocabulary
+    of ``find_vocab(bpe_path, checkpoints_dir)``.  A text longer than the context raises RuntimeError like ``clip.tokenize``."""
+    _require_cuda(device)
+    clip_sd = clip_state_dict if clip_state_dict is not None else _load_clip_sd(clip_model_name, checkpoints_dir)
+    embeds, _ = _encode_text_device([txt], clip_sd, find_vocab(bpe_path, checkpoints_dir), device)
+    return embeds, weight
+
+
 def _lpips_sd(given):
     """LPIPS(net='vgg') weights in upstream key layout: passed in, or taken from the ``lpips`` package when it is installed"""
     if given is not None:
@@ -178,7 +229,7 @@ def clip_guided_diffusion(
     # --- additions of this framework (all optional)
     unet_state_dict: dict = None, clip_state_dict: dict = None, target_embeds: th.Tensor = None, weights: th.Tensor = None,
     lpips_state_dict: dict = None, cutout_resize: str = "pool",
-    rank: int = 0, world_size: int = 1,
+    rank: int = 0, world_size: int = 1, text_encoder: str = "auto", bpe_path: str = None,
 ):
     if len(device) == 0:
         device = "cuda"
@@ -191,6 +242,8 @@ def clip_guided_diffusion(
         check_local(path)
     if wandb_project is not None:
         raise NotImplementedError("W&B logging is outside the hot path (SURVEY section 2)")
+    if text_encoder not in ("auto", "clip", "device"):
+        raise ValueError(f"text_encoder={text_encoder!r}: expected 'auto', 'clip' or 'device'")
     th.manual_seed(seed)
     if not use_magnitude and image_size == 64:  # cgd/cgd.py:72-74
         use_magnitude = True
@@ -201,7 +254,11 @@ def clip_guided_diffusion(
         # text prompts first, then every image prompt's cutn embeddings (cgd/cgd.py:86-98); an image-only run needs no text tower
         embeds, weights = [], []
         if prompts or not image_prompts:
-            e, w = _encode_text(prompts, clip_model_name, device)
+            vocab = _text_encoder_choice(text_encoder, bpe_path, checkpoints_dir) if prompts else None
+            if vocab is not None:  # one forward-only text tower from the visual tower's state_dict, released here
+                e, w = _encode_text_device(prompts, clip_sd, vocab, device)
+            else:
+                e, w = _encode_text(prompts, clip_model_name, device)
             embeds.append(e)
             weights += [float(v) for v in w]
         if image_prompts:

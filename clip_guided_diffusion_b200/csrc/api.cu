@@ -66,6 +66,8 @@ static int dispatch(const CgdOp& op, const ConvTcLaunch* conv, cudaStream_t st) 
     case CGD_OP_CUTOUTS_AUG_FWD: return launch_cutouts_aug_fwd(op, st);
     case CGD_OP_CUTOUTS_AUG_BWD: return launch_cutouts_aug_bwd(op, st);
     case CGD_OP_RESIZE_AXIS: return launch_resize_axis(op, st);
+    case CGD_OP_TOKEN_EMBED: return launch_token_embed(op, st);
+    case CGD_OP_ROW_GATHER: return launch_row_gather(op, st);
     case CGD_OP_SEED_QUANT: return launch_seed_quant(op, st);
     case CGD_OP_MAG_CLAMP: return launch_mag_clamp(op, st);
     case CGD_OP_ATTNPOOL_EMBED_FWD: return launch_attnpool_embed_fwd(op, st);

@@ -11,13 +11,16 @@
 namespace cgd {
 
 int attn_small_supported(int64_t T);                         // attention_small.cu: one 64-key tile per head on warp MMAs
-int launch_attn_small_fwd(const AttnArgs& a, cudaStream_t st);
+int launch_attn_small_fwd(const AttnArgs& a, bool causal, cudaStream_t st);
 int launch_attn_small_bwd(const AttnArgs& a, cudaStream_t st);
-int launch_attn_flash_fwd(const AttnArgs& a, int nc, cudaStream_t st);  // attention_flash.cu: flash attention, head dim 64 * nc (any T)
+int launch_attn_flash_fwd(const AttnArgs& a, int nc, bool causal, cudaStream_t st);  // attention_flash.cu: flash attention, head dim 64 * nc (any T)
 int launch_attn_flash_bwd(const AttnArgs& a, int nc, cudaStream_t st);
 
 static int attn_args(const CgdOp& op, bool bwd, AttnArgs& a) {
   const int64_t d = op.i[3];
+  // flags 1 (forward only) = causal; nothing differentiates a causal attention, so the backward takes no flags
+  if (!bwd) CGD_CHECK_ARG((op.flags & ~1) == 0, "attention: flags %d unsupported (1 = causal)", (int)op.flags);
+  else CGD_CHECK_ARG(op.flags == 0, "attention bwd: flags %d unsupported (no causal backward)", (int)op.flags);
   CGD_CHECK_ARG(d == 64 || d == 128 || d == 192 || d == 256, "attention: head dim %lld unsupported (64, 128, 192, 256)", (long long)d);
   CGD_CHECK_ARG((int)op.i[0] > 0 && (int)op.i[1] > 0 && (int)op.i[2] > 0, "attention: bad dims");
   for (int k = 4; k <= 9; ++k) CGD_CHECK_ARG(op.i[k] % 8 == 0, "attention: strides must be multiples of 8 elements");
@@ -45,7 +48,8 @@ int attn_bwd_num_launches(const CgdOp& op) { return attn_small(op) ? 1 : 2; }
 int launch_attn_fwd(const CgdOp& op, cudaStream_t st) {
   AttnArgs a;
   if (int rc = attn_args(op, false, a)) return rc;
-  return attn_small(op) ? launch_attn_small_fwd(a, st) : launch_attn_flash_fwd(a, (int)(op.i[3] / AS_T), st);
+  const bool causal = op.flags & 1;
+  return attn_small(op) ? launch_attn_small_fwd(a, causal, st) : launch_attn_flash_fwd(a, (int)(op.i[3] / AS_T), causal, st);
 }
 
 int launch_attn_bwd(const CgdOp& op, cudaStream_t st) {

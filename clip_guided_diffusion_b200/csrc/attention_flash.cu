@@ -63,7 +63,9 @@ __device__ __forceinline__ void af_mm_nk(float (&acc)[8][4], const __half* X, co
 }
 
 // ------------------------------------------------------------------------------------------------ forward
-template <int NC>
+// CAUSAL: query i attends to keys j <= i only (the CLIP text tower).  A CTA's key loop then ends at the diagonal tile (key tile
+// blockIdx.x), the only tile that needs masking.  Key tile 0 always holds key 0, so the running max is finite after it.
+template <int NC, bool CAUSAL>
 __global__ void __launch_bounds__(128) attn_flash_fwd_kernel(const AttnArgs a) {
   // Q | K0 | K1 | V0 | V1, NC tiles each.  NC = 1 (45 KB) fits static shared memory, which compiles to faster code for d = 64;
   // larger NC need the dynamic allocation.
@@ -83,7 +85,7 @@ __global__ void __launch_bounds__(128) attn_flash_fwd_kernel(const AttnArgs a) {
   const int q0 = blockIdx.x * AS_T, h = blockIdx.y, b = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t qoff = (int64_t)b * a.qbs + (int64_t)h * a.qhs;
-  const int n_kt = (a.T + AS_T - 1) / AS_T;
+  const int n_kt = CAUSAL ? min((a.T + AS_T - 1) / AS_T, (int)blockIdx.x + 1) : (a.T + AS_T - 1) / AS_T;
   af_load_async<NC>(Qs, a.q + qoff, a.qrs, q0, a.T);
   af_load_async<NC>(Ks, a.k + qoff, a.qrs, 0, a.T);
   af_load_async<NC>(Vs, a.v + qoff, a.qrs, 0, a.T);
@@ -114,8 +116,16 @@ __global__ void __launch_bounds__(128) attn_flash_fwd_kernel(const AttnArgs a) {
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const bool ok = k0 + j * 8 + cb + e < a.T;
-        s[j][e] = ok ? s[j][e] * a.scale : -INFINITY;
-        s[j][2 + e] = ok ? s[j][2 + e] * a.scale : -INFINITY;
+        bool ok0 = ok, ok1 = ok;
+        if constexpr (CAUSAL) {
+          // diagonal tile (q0 == k0): key column c is masked for the tile's query rows < c
+          const int col = j * 8 + cb + e, ra = r0 + (lane >> 2);
+          const bool diag = kt == (int)blockIdx.x;
+          ok0 = ok && !(diag && col > ra);
+          ok1 = ok && !(diag && col > ra + 8);
+        }
+        s[j][e] = ok0 ? s[j][e] * a.scale : -INFINITY;
+        s[j][2 + e] = ok1 ? s[j][2 + e] * a.scale : -INFINITY;
         mx0 = fmaxf(mx0, s[j][e]);
         mx1 = fmaxf(mx1, s[j][2 + e]);
       }
@@ -124,7 +134,7 @@ __global__ void __launch_bounds__(128) attn_flash_fwd_kernel(const AttnArgs a) {
     mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
     mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
     mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
-    const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);  // finite: every key tile holds at least one valid key
+    const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);  // finite: every key tile holds at least one valid key per row
     const float al0 = __expf(m0 - mn0), al1 = __expf(m1 - mn1);
     float rs0 = 0.f, rs1 = 0.f;
 #pragma unroll
@@ -357,15 +367,15 @@ __global__ void __launch_bounds__(128) attn_flash_bwd_kernel(const AttnArgs a, i
 }
 
 // ------------------------------------------------------------------------------------------------ host
-template <int NC>
+template <int NC, bool CAUSAL>
 static int af_fwd(const AttnArgs& a, cudaStream_t st) {
   constexpr int smem = NC == 1 ? 0 : 5 * NC * AS_TILE * (int)sizeof(__half);  // dynamic shared memory
   static DeviceOnce set;
   if (set.needed()) {
-    CGD_CUDA(cudaFuncSetAttribute(attn_flash_fwd_kernel<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    CGD_CUDA(cudaFuncSetAttribute(attn_flash_fwd_kernel<NC, CAUSAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     set.mark();
   }
-  CGD_CUDA(launch_pdl(attn_flash_fwd_kernel<NC>, dim3((unsigned)ceil_div(a.T, AS_T), a.heads, a.B), dim3(128), smem, st, a));
+  CGD_CUDA(launch_pdl(attn_flash_fwd_kernel<NC, CAUSAL>, dim3((unsigned)ceil_div(a.T, AS_T), a.heads, a.B), dim3(128), smem, st, a));
   return 0;
 }
 
@@ -385,12 +395,12 @@ static int af_bwd(const AttnArgs& a, cudaStream_t st) {
   return 0;
 }
 
-int launch_attn_flash_fwd(const AttnArgs& a, int nc, cudaStream_t st) {
+int launch_attn_flash_fwd(const AttnArgs& a, int nc, bool causal, cudaStream_t st) {
   switch (nc) {
-    case 1: return af_fwd<1>(a, st);
-    case 2: return af_fwd<2>(a, st);
-    case 3: return af_fwd<3>(a, st);
-    case 4: return af_fwd<4>(a, st);
+    case 1: return causal ? af_fwd<1, true>(a, st) : af_fwd<1, false>(a, st);
+    case 2: return causal ? af_fwd<2, true>(a, st) : af_fwd<2, false>(a, st);
+    case 3: return causal ? af_fwd<3, true>(a, st) : af_fwd<3, false>(a, st);
+    case 4: return causal ? af_fwd<4, true>(a, st) : af_fwd<4, false>(a, st);
     default: break;
   }
   CGD_CHECK_ARG(false, "attention: head dim %d unsupported (64, 128, 192, 256)", nc * AS_T);

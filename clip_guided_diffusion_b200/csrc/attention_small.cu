@@ -5,7 +5,7 @@
 // 8x8 UNet level (64 tokens) (SURVEY.md K4, K14).  Why a separate kernel: these problems are one 64x64 tile per head -- the
 // flash kernels of attention_flash.cu need two launches for the backward.  Here the
 // whole backward -- S, P, dP, dS, dQ, dK, dV -- is one launch; P and dS go through shared memory once (fp16, like the
-// reference's fp16 attention weights) to feed the transposed products.
+// reference's fp16 attention weights) to feed the transposed products.  The forward also comes causal (the CLIP text tower).
 #include <cuda_fp16.h>
 
 #include "attn_mma.cuh"
@@ -15,6 +15,8 @@
 
 namespace cgd {
 
+// CAUSAL: query i attends to keys j <= i only (the CLIP text tower)
+template <bool CAUSAL>
 __global__ void __launch_bounds__(128) attn_small_fwd_kernel(const AttnArgs a) {
   __shared__ __align__(16) __half Qs[AS_TILE], Ks[AS_TILE], Vs[AS_TILE];
   pdl_wait();
@@ -30,7 +32,7 @@ __global__ void __launch_bounds__(128) attn_small_fwd_kernel(const AttnArgs a) {
   if (r0 >= a.T) return;
   float s[8][4], lse0, lse1;
   as_mm_nk(s, Qs, Ks, r0, lane);
-  as_softmax(s, a.T, a.scale, lane, lse0, lse1);
+  as_softmax<CAUSAL>(s, a.T, a.scale, lane, lse0, lse1, r0);
   if (a.lse && (lane & 3) == 0) {
     const int ra = r0 + (lane >> 2);
     float* l = a.lse + ((int64_t)b * a.heads + h) * a.T;
@@ -102,8 +104,9 @@ __global__ void __launch_bounds__(128) attn_small_bwd_kernel(const AttnArgs a) {
 
 int attn_small_supported(int64_t T) { return T >= 1 && T <= AS_T; }
 
-int launch_attn_small_fwd(const AttnArgs& a, cudaStream_t st) {
-  CGD_CUDA(launch_pdl(attn_small_fwd_kernel, dim3(a.heads, a.B), dim3(128), 0, st, a));
+int launch_attn_small_fwd(const AttnArgs& a, bool causal, cudaStream_t st) {
+  if (causal) CGD_CUDA(launch_pdl(attn_small_fwd_kernel<true>, dim3(a.heads, a.B), dim3(128), 0, st, a));
+  else CGD_CUDA(launch_pdl(attn_small_fwd_kernel<false>, dim3(a.heads, a.B), dim3(128), 0, st, a));
   return 0;
 }
 int launch_attn_small_bwd(const AttnArgs& a, cudaStream_t st) {

@@ -128,17 +128,21 @@ __device__ __forceinline__ void as_mm_t_kn(float (&acc)[8][4], const __half* X, 
   }
 }
 
-// Row softmax of the warp's 16 x 64 score fragment (rows lane/4 and lane/4 + 8), keys >= T masked; returns P in `s`.
-__device__ __forceinline__ void as_softmax(float (&s)[8][4], int T, float scale, int lane, float& lse0, float& lse1) {
+// Row softmax of the warp's 16 x 64 score fragment (rows r0 + lane/4 and r0 + lane/4 + 8), keys >= T masked, and with CAUSAL
+// also keys after the row's query; returns P in `s`.
+template <bool CAUSAL = false>
+__device__ __forceinline__ void as_softmax(float (&s)[8][4], int T, float scale, int lane, float& lse0, float& lse1, int r0 = 0) {
   const int cbase = (lane & 3) * 2;
+  const int ra = r0 + (lane >> 2);
   float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
-      const bool ok = j * 8 + cbase + e < T;
-      s[j][e] = ok ? s[j][e] * scale : -INFINITY;
-      s[j][2 + e] = ok ? s[j][2 + e] * scale : -INFINITY;
+      const int col = j * 8 + cbase + e;
+      const bool ok = col < T;
+      s[j][e] = ok && (!CAUSAL || col <= ra) ? s[j][e] * scale : -INFINITY;  // key 0 is never masked: the row max stays finite
+      s[j][2 + e] = ok && (!CAUSAL || col <= ra + 8) ? s[j][2 + e] * scale : -INFINITY;
       mx0 = fmaxf(mx0, s[j][e]);
       mx1 = fmaxf(mx1, s[j][2 + e]);
     }

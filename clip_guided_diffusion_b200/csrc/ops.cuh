@@ -43,6 +43,8 @@ int launch_cutouts_rr_bwd(const CgdOp& op, cudaStream_t st);
 int launch_cutouts_aug_fwd(const CgdOp& op, cudaStream_t st);
 int launch_cutouts_aug_bwd(const CgdOp& op, cudaStream_t st);
 int launch_resize_axis(const CgdOp& op, cudaStream_t st);
+int launch_token_embed(const CgdOp& op, cudaStream_t st);
+int launch_row_gather(const CgdOp& op, cudaStream_t st);
 int launch_seed_quant(const CgdOp& op, cudaStream_t st);
 int launch_mag_clamp(const CgdOp& op, cudaStream_t st);
 int launch_attnpool_embed_fwd(const CgdOp& op, cudaStream_t st);

@@ -553,9 +553,10 @@ class Plan:
         return y
 
     # ------------------------------------------------------------------ attention (head dim 64; 128 / 192 / 256 for the 128^2 checkpoint)
-    def attention(self, qkv: Act, heads: int, T: int, nbatch: int, legacy_order: bool, name="attn") -> Act:
+    def attention(self, qkv: Act, heads: int, T: int, nbatch: int, legacy_order: bool, causal: bool = False, name="attn") -> Act:
         """qkv: [nbatch*T rows, 3C].  legacy_order: per-head [q|k|v] interleave (UNet QKVAttentionLegacy);
-        otherwise [q heads | k heads | v heads] (QKVAttention, nn.MultiheadAttention)."""
+        otherwise [q heads | k heads | v heads] (QKVAttention, nn.MultiheadAttention).  causal: query i attends to keys <= i
+        (ATTN_FWD flags 1, the CLIP text tower); forward only."""
         C = qkv.C // 3
         d = C // heads
         assert d in (64, 128, 192, 256), f"attention kernels support head dims 64 / 128 / 192 / 256, got {d}"
@@ -570,12 +571,14 @@ class Plan:
         q = (qkv.buf, qkv.eoff + qo)
         k = (qkv.buf, qkv.eoff + ko)
         v = (qkv.buf, qkv.eoff + vo)
-        self.emit("ATTN_FWD", i=ii, f=[scale], p=[q, k, v, self._ap(out), self._bp(lse)], tag=name)
+        self.emit("ATTN_FWD", flags=1 if causal else 0, i=ii, f=[scale], p=[q, k, v, self._ap(out), self._bp(lse)], tag=name)
 
         def bwd():
             do = self.grad_of(out)
             if do is None:
                 return
+            if causal:
+                raise NotImplementedError(f"{name}: a causal attention has no backward (ATTN_BWD takes no flags)")
             assert do.ld == out.ld
             dqkv = Act(self.new(nbatch * T * qkv.ld, "h", "d_" + name), 0, qkv.N, qkv.H, qkv.W, qkv.C, qkv.ld)
             delta = self.new(nbatch * heads * T, "f", name + "_delta")

@@ -84,6 +84,20 @@ def vit_param_shapes(cfg: ViTConfig) -> dict:
     return sh
 
 
+def text_param_shapes(cfg) -> dict:
+    """CLIP text tower (``text.TextConfig``) in upstream key layout: the keys of a full CLIP state_dict outside ``visual.*``"""
+    w = cfg.width
+    sh = {"token_embedding.weight": (cfg.vocab_size, w), "positional_embedding": (cfg.context_length, w)}
+    for i in range(cfg.layers):
+        p = f"transformer.resblocks.{i}"
+        sh.update({p + ".attn.in_proj_weight": (3 * w, w), p + ".attn.in_proj_bias": (3 * w,), p + ".attn.out_proj.weight": (w, w),
+                   p + ".attn.out_proj.bias": (w,), p + ".ln_1.weight": (w,), p + ".ln_1.bias": (w,), p + ".mlp.c_fc.weight": (4 * w, w),
+                   p + ".mlp.c_fc.bias": (4 * w,), p + ".mlp.c_proj.weight": (w, 4 * w), p + ".mlp.c_proj.bias": (w,),
+                   p + ".ln_2.weight": (w,), p + ".ln_2.bias": (w,)})
+    sh.update({"ln_final.weight": (w,), "ln_final.bias": (w,), "text_projection": (w, cfg.output_dim)})
+    return sh
+
+
 def rn_param_shapes(cfg) -> dict:
     """CLIP ModifiedResNet visual tower ([3P] clip/model.py) in upstream key layout, BatchNorm buffers included"""
     w = cfg.width

@@ -93,13 +93,13 @@ enum {
   CGD_OP_UP2 = 7,
   /* c = a + b on [rows, C] fp16: p0 a p1 b p2 c ; i0 rows i1 C i2 lda i3 ldb i4 ldc */
   CGD_OP_ADD = 8,
-  /* Multi-head softmax attention forward, head dim 64 (SURVEY K4, K14).
+  /* Multi-head softmax attention forward, head dim 64 / 128 / 192 / 256 (SURVEY K4, K14).
    * p0 q p1 k p2 v p3 out p4 lse(f [B,heads,T]) ; i0 B i1 heads i2 T i3 d
    * i4 qkv batch stride i5 qkv row stride i6 qkv head stride i7 out batch stride i8 out row stride i9 out head stride
-   * f0 softmax scale (applied to q.k) */
+   * f0 softmax scale (applied to q.k) ; flags 1 = causal: key j > i is masked for query i (the CLIP text tower) */
   CGD_OP_ATTN_FWD = 9,
   /* backward: p0 q p1 k p2 v p3 out p4 dout p5 lse p6 dq p7 dk p8 dv p9 delta ws(f [B,heads,T])
-   * i/f as forward (dq/dk/dv use the qkv strides, dout the out strides) */
+   * i/f as forward (dq/dk/dv use the qkv strides, dout the out strides) ; flags 0 (there is no causal backward) */
   CGD_OP_ATTN_BWD = 10,
   /* Small-M fp32 linear: y[M,N] (=|+=) act(x[M,K]) @ W[N,K]^T + b.  time_embed / emb_layers / CLIP head (SURVEY K8, K16).
    * p0 x(f|h) p1 W(f|h) p2 b(f)|0 p3 y(f|h) p4 scatter(i32 [N,2] = element offset of row 0, row stride)|0 ; i0 M i1 K (% 8 == 0)
@@ -232,6 +232,14 @@ enum {
    * in tap order.  p0 in(f [planes, H, W]) p1 out(f [planes, O, W] for axis 0, [planes, H, O] for axis 1) p2 left(i32 [O])
    * p3 weights(f [O, T]) ; i0 planes i1 H i2 W i3 axis (0 = H, 1 = W) i4 O i5 T */
   CGD_OP_RESIZE_AXIS = 52,
+  /* CLIP text tower input ([3P] clip/model.py encode_text): x[n,t,:] = fp16(table[ids[n,t],:] + pos[t,:]), the sum in fp32.
+   * p0 ids(i32 [n,T]) p1 table(h [V,w]) p2 pos(f [T,w]) p3 x(h [n,T,w]) ; i0 n i1 T i2 w (% 8 == 0) i3 V.
+   * An id outside [0, V) gives a row of NaNs (never a read outside the table); callers check ids on the host. */
+  CGD_OP_TOKEN_EMBED = 53,
+  /* y[i,:] = x[idx[i],:] on fp16 rows (the end-of-text token of every sequence: idx[i] = i * T + eot_i).
+   * p0 x(h [n_src rows, row stride i2]) p1 idx(i32 [rows], 4-byte aligned) p2 y(h [rows, row stride i3]) ; i0 rows i1 w (% 8 == 0) i2 ldx i3 ldy
+   * i4 n_src.  An index outside [0, n_src) gives a row of NaNs. */
+  CGD_OP_ROW_GATHER = 54,
   CGD_OP__COUNT
 };
 
