@@ -21,6 +21,12 @@ path (cgd/clip_util.py:104-108), by one of two text towers (``text_encoder=``):
 - ``"auto"`` (default): the ``clip`` package if it imports, else the device tower if the vocabulary file is found, else the ``clip``
   path, which raises without the package.
 Or pass ``target_embeds`` / ``weights`` directly.  Image prompts use this package's own CLIP visual tower and never import ``clip``.
+
+Several CLIP towers (``clip_model_name=["ViT-B/32", "ViT-B/16", "RN50"]``) guide one run together: each tower cuts its own
+``num_cutouts`` windows at its own resolution, gets its own text and image targets, and the CLIP losses are summed (the reference's CLIP
+block once per tower; tv / range / sat / LPIPS once).  A name is a tower name or a path to a CLIP checkpoint file (``.pt``: a TorchScript
+archive or a plain state_dict, the architecture read from its keys).  With several towers, ``target_embeds=`` is one ``[P, D_m]`` tensor
+per tower and ``clip_state_dict=`` one state_dict (or None) per tower; ``use_augs`` and ``cutout_resize="lanczos3"`` take one tower.
 """
 from __future__ import annotations
 
@@ -192,8 +198,27 @@ def _tower_config(clip_sd: dict):
     return vit_config_from_state_dict(clip_sd)
 
 
+def _is_checkpoint_path(clip_model_name) -> bool:
+    """a CLIP checkpoint file rather than a tower name (the reference's `clip.load(path)` fallback, cgd/clip_util.py:52-56)"""
+    return str(clip_model_name).endswith(".pt") or os.path.isfile(str(clip_model_name))
+
+
+def _load_clip_file(path):
+    """a CLIP checkpoint file -> state_dict: a TorchScript archive first, then a plain state_dict (as `_load_clip_sd`)"""
+    if not os.path.isfile(path):
+        raise FileNotFoundError(f"CLIP checkpoint {path} not found")
+    try:
+        return th.jit.load(path, map_location="cpu").state_dict()
+    except RuntimeError:
+        return th.load(path, map_location="cpu")
+
+
 def _clip_tower(clip_model_name, clip_state_dict, checkpoints_dir):
-    """-> (CLIP state_dict, visual tower config): the given state_dict's own architecture, or the named tower's checkpoint"""
+    """-> (CLIP state_dict, visual tower config): the given state_dict's own architecture, a checkpoint file's (a path) or the named
+    tower's checkpoint"""
+    if clip_state_dict is None and _is_checkpoint_path(clip_model_name):
+        clip_sd = _load_clip_file(str(clip_model_name))
+        return clip_sd, _tower_config(clip_sd)
     clip_sd = clip_state_dict if clip_state_dict is not None else _load_clip_sd(clip_model_name, checkpoints_dir)
     towers = {**VIT_CONFIGS, **RN_CONFIGS}
     if clip_state_dict is None and clip_model_name not in towers:
@@ -212,6 +237,25 @@ def encode_image_prompt(image: str, weight: float, diffusion_size: int, num_cuto
     return ImagePromptEncoder(cfg, clip_sd, num_cutouts, device).encode(image, weight, diffusion_size)
 
 
+def _tower_list(clip_model_name, clip_state_dict):
+    """-> (names, state_dicts): `clip_model_name` is one name or a non-empty sequence of them; `clip_state_dict` None, one
+    state_dict (one tower) or a sequence of the names' length"""
+    names = [clip_model_name] if isinstance(clip_model_name, (str, os.PathLike)) else list(clip_model_name)
+    if not names:
+        raise ValueError("clip_model_name: a tower name, a checkpoint path or a non-empty sequence of them")
+    if clip_state_dict is None:
+        sds = [None] * len(names)
+    elif isinstance(clip_state_dict, dict):
+        if len(names) != 1:
+            raise ValueError(f"{len(names)} CLIP towers: clip_state_dict must be a sequence of {len(names)} state_dicts (or None)")
+        sds = [clip_state_dict]
+    else:
+        sds = list(clip_state_dict)
+        if len(sds) != len(names):
+            raise ValueError(f"{len(names)} CLIP towers but {len(sds)} clip_state_dict entries")
+    return names, sds
+
+
 def _require_cuda(device):
     if not str(device).startswith("cuda") or not th.cuda.is_available():
         raise RuntimeError("clip_guided_diffusion_b200 runs the sampling step on a CUDA (sm_90a, H100) device only; there is no CPU path")
@@ -222,7 +266,7 @@ def clip_guided_diffusion(
     clip_guidance_scale: int = 1000, tv_scale: float = 150, range_scale: float = 50, sat_scale: float = 0, init_scale: float = 0,
     batch_size: int = 1, init_image=None, class_cond: bool = True, cutout_power: float = 1.0, timestep_respacing: str = "1000",
     seed: int = 0, diffusion_steps: int = 1000, skip_timesteps: int = 0, checkpoints_dir: str = CACHE_PATH,
-    clip_model_name: str = "ViT-B/32", randomize_class: bool = True, prefix_path=Path("./outputs"), save_frequency: int = 25,
+    clip_model_name: "str | list[str]" = "ViT-B/32", randomize_class: bool = True, prefix_path=Path("./outputs"), save_frequency: int = 25,
     noise_schedule: str = "linear", dropout: float = 0.0, device: str = "", wandb_project: str = None, wandb_entity: str = None,
     use_augs: bool = False, use_magnitude: bool = False, height_offset: int = 0, width_offset: int = 0, progress: bool = True,
     reduce_clip: bool = False, progressive_cutout: bool = False, cached_cutouts: bool = False,
@@ -234,6 +278,20 @@ def clip_guided_diffusion(
     if len(device) == 0:
         device = "cuda"
     _require_cuda(device)
+    names, clip_sds = _tower_list(clip_model_name, clip_state_dict)
+    T = len(names)
+    if T > 1 and use_augs:
+        raise NotImplementedError("use_augs with several CLIP towers (the augmentation parameters are drawn for one tower's cutouts)")
+    if T > 1 and cutout_resize == "lanczos3":
+        raise NotImplementedError("cutout_resize='lanczos3' with several CLIP towers (the resampling tables are built for one tower)")
+    if target_embeds is not None:
+        if isinstance(target_embeds, th.Tensor):
+            if T > 1:
+                raise ValueError(f"{T} CLIP towers: target_embeds= must be a sequence of {T} [P, D_m] tensors, one per tower")
+            target_embeds = [target_embeds]
+        target_embeds = list(target_embeds)
+        if len(target_embeds) != T or len({int(e.shape[0]) for e in target_embeds}) != 1:
+            raise ValueError(f"target_embeds=: one [P, D_m] tensor per CLIP tower ({T}), the same P each")
     if image_prompts and target_embeds is not None:
         raise NotImplementedError("target_embeds= is the complete target set: with image prompts, encode them with encode_image_prompt() "
                                   "and append the embeddings and weights to target_embeds= / weights= instead of passing image_prompts=")
@@ -249,30 +307,35 @@ def clip_guided_diffusion(
         use_magnitude = True
     Path(prefix_path).mkdir(parents=True, exist_ok=True)
 
-    clip_sd, vit_cfg = _clip_tower(clip_model_name, clip_state_dict, checkpoints_dir)
+    towers = [_clip_tower(n, sd, checkpoints_dir) for n, sd in zip(names, clip_sds)]  # [(state_dict, visual config)] in tower order
     if target_embeds is None:
-        # text prompts first, then every image prompt's cutn embeddings (cgd/cgd.py:86-98); an image-only run needs no text tower
-        embeds, weights = [], []
+        # text prompts first, then every image prompt's cutn embeddings (cgd/cgd.py:86-98); an image-only run needs no text tower.
+        # Every tower encodes the same prompts with its own text half / visual tower; the weights are the same for every tower.
+        embeds, weights = [[] for _ in towers], []
         if prompts or not image_prompts:
             vocab = _text_encoder_choice(text_encoder, bpe_path, checkpoints_dir) if prompts else None
-            if vocab is not None:  # one forward-only text tower from the visual tower's state_dict, released here
-                e, w = _encode_text_device(prompts, clip_sd, vocab, device)
-            else:
-                e, w = _encode_text(prompts, clip_model_name, device)
-            embeds.append(e)
+            for m, (name, (clip_sd, _)) in enumerate(zip(names, towers)):
+                if vocab is not None:  # one forward-only text tower from the visual tower's state_dict, released here
+                    e, w = _encode_text_device(prompts, clip_sd, vocab, device)
+                else:
+                    e, w = _encode_text(prompts, name, device)
+                embeds[m].append(e)
             weights += [float(v) for v in w]
         if image_prompts:
-            # one forward-only tower for every image prompt, released before the engine is built; its cutout windows come from the
-            # CPU generator after the seed and before cache_coordinates / the loop, where the reference draws them
-            encoder = ImagePromptEncoder(vit_cfg, clip_sd, num_cutouts, device)
-            for path, w in image_prompts:
-                e, ws = encoder.encode(path, w, image_size)
-                embeds.append(e)
-                weights += ws
-            del encoder
-        target_embeds, weights = th.cat([e.to(device) for e in embeds]), th.tensor(weights)
+            # tower-major: one forward-only tower for every image prompt, released before the next tower's (and before the engine)
+            # is built; the cutout windows come from the CPU generator after the seed and before cache_coordinates / the loop, where
+            # the reference draws them
+            for m, (clip_sd, vit_cfg) in enumerate(towers):
+                encoder = ImagePromptEncoder(vit_cfg, clip_sd, num_cutouts, device)
+                for path, w in image_prompts:
+                    e, ws = encoder.encode(path, w, image_size)
+                    embeds[m].append(e)
+                    if m == 0:
+                        weights += ws
+                del encoder
+        target_embeds, weights = [th.cat([e.to(device) for e in em]) for em in embeds], th.tensor(weights)
     if weights is None:  # target_embeds= given without weights=: every prompt weighs 1 (parse_prompt's default)
-        weights = th.ones(target_embeds.shape[0])
+        weights = th.ones(target_embeds[0].shape[0])
     weights = th.as_tensor(weights, dtype=th.float32)
     if weights.sum().abs() < 1e-3:
         raise RuntimeError("The weights must not sum to 0.")
@@ -292,18 +355,21 @@ def clip_guided_diffusion(
     assert local_b * world_size == batch_size, "batch_size must divide evenly over the ranks"
     # progressive_cutout runs max(4, n // 4), max(8, n // 2), n cutouts (cgd/cgd.py:167-175): the middle count exceeds n when n < 16
     counts = CondFnB200.progressive_counts(num_cutouts) if progressive_cutout else (num_cutouts,)
-    engine = GuidedStepB200(unet_cfg, unet_sd, vit_cfg, clip_sd, batch=local_b, height=H, width=W, num_cutouts=max(counts),
-                            max_prompts=target_embeds.shape[0], clip_guidance_scale=clip_guidance_scale, tv_scale=tv_scale,
+    cfgs, sds = [cfg for _, cfg in towers], [sd for sd, _ in towers]
+    engine = GuidedStepB200(unet_cfg, unet_sd, cfgs[0] if T == 1 else cfgs, sds[0] if T == 1 else sds, batch=local_b, height=H, width=W,
+                            num_cutouts=max(counts), max_prompts=target_embeds[0].shape[0], clip_guidance_scale=clip_guidance_scale, tv_scale=tv_scale,
                             range_scale=range_scale, sat_scale=sat_scale, use_magnitude=use_magnitude, device=device, rank=rank,
                             world_size=world_size,
                             cutn_variants=tuple(c for c in counts if c != max(counts)),
                             lpips_sd=_lpips_sd(lpips_state_dict) if (init_image is not None and init_scale != 0) else None,
                             init_scale=init_scale, cutout_resize=cutout_resize, use_augs=use_augs)
-    engine.set_targets(target_embeds, weights)
-    make_cutouts = MakeCutouts(cut_size=vit_cfg.input_resolution, num_cutouts=num_cutouts, cutout_size_power=cutout_power, use_augs=use_augs)
+    engine.set_targets(target_embeds[0] if T == 1 else target_embeds, weights)
+    make_cutouts = [MakeCutouts(cut_size=cfg.input_resolution, num_cutouts=num_cutouts, cutout_size_power=cutout_power, use_augs=use_augs)
+                    for cfg in cfgs]
     if cached_cutouts:
-        make_cutouts.cache_coordinates(W, H)  # cgd/cgd.py:113
-    cond_fn = CondFnB200(engine, diffusion, make_cutouts, cached_cutouts=cached_cutouts, reduce_clip=reduce_clip,
+        for mk in make_cutouts:  # cgd/cgd.py:113, once per tower in tower order
+            mk.cache_coordinates(W, H)
+    cond_fn = CondFnB200(engine, diffusion, make_cutouts[0] if T == 1 else make_cutouts, cached_cutouts=cached_cutouts, reduce_clip=reduce_clip,
                          progressive_cutout=progressive_cutout)
 
     init_tensor = None

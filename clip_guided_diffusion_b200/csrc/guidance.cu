@@ -67,6 +67,9 @@ __global__ void cutouts_fwd_kernel(const float* __restrict__ x, const int* __res
 }
 
 // ---------------------------------------------------------------- cutouts backward (gather, no atomics)
+// ACC (CUTOUTS_BWD flags 2): dx += the cutout gradient instead of dx = it -- the CLIP towers of an ensemble after the first add
+// theirs in launch order.  The sum is an explicit __fadd_rn, so dx ends bitwise equal to old + what ACC = false stores.
+template <bool ACC>
 __global__ void cutouts_bwd_kernel(const __half* __restrict__ dpatch, const int* __restrict__ coords, float* __restrict__ dx, int B, int H,
                                    int W, int cutn, int cs, int P, int Kpad, float3 stdv, float scale) {
   pdl_wait();
@@ -104,7 +107,11 @@ __global__ void cutouts_bwd_kernel(const __half* __restrict__ dpatch, const int*
         }
       }
     }
-    dx[idx] = acc * (0.5f / sd) * scale;
+    const float v = acc * (0.5f / sd) * scale;
+    if constexpr (ACC)
+      dx[idx] = __fadd_rn(dx[idx], v);
+    else
+      dx[idx] = v;
   }
 }
 
@@ -191,6 +198,7 @@ cutouts_fwd_rows_kernel(const float* __restrict__ x, const int* __restrict__ coo
 constexpr int CUT_MAX_CUTN = 128;
 constexpr int CUT_BWD_THREADS = 128;  // columns per block: H * ceil(W / 128) blocks per image keep >= 3 CTAs per SM at 256 x 256
 constexpr int CUT_MAX_ROWS = 8;  // output rows whose bins contain one input row: <= ceil(cs / S) + 1 (up-sampling 64 -> 224: 5)
+template <bool ACC>  // as cutouts_bwd_kernel
 __global__ void __launch_bounds__(CUT_BWD_THREADS)
 cutouts_bwd_rows_kernel(const __half* __restrict__ dpatch, const int* __restrict__ coords, float* __restrict__ dx, int B, int H, int W, int cutn,
                         int cs, int P, int Kpad, float3 stdv, float scale) {
@@ -262,7 +270,14 @@ cutouts_bwd_rows_kernel(const __half* __restrict__ dpatch, const int* __restrict
       }
     }
 #pragma unroll
-    for (int c = 0; c < 3; ++c) dx[(((int64_t)b * 3 + c) * H + yg) * W + xg] = acc[c] * (0.5f / sd3[c]) * scale;
+    for (int c = 0; c < 3; ++c) {
+      if constexpr (ACC) {
+        float* d = dx + (((int64_t)b * 3 + c) * H + yg) * W + xg;
+        *d = __fadd_rn(*d, acc[c] * (0.5f / sd3[c]) * scale);
+      } else {
+        dx[(((int64_t)b * 3 + c) * H + yg) * W + xg] = acc[c] * (0.5f / sd3[c]) * scale;
+      }
+    }
   }
 }
 
@@ -407,16 +422,19 @@ int launch_cutouts_fwd(const CgdOp& op, cudaStream_t st) {
 }
 int launch_cutouts_bwd(const CgdOp& op, cudaStream_t st) {
   if (int rc = cutout_check(op)) return rc;
+  CGD_CHECK_ARG(op.flags == 0 || op.flags == 2, "cutouts_bwd: flags must be 0 (store) or 2 (accumulate), got %d", op.flags);
+  const bool acc = op.flags & 2;
   const int64_t B = op.i[0], H = op.i[1], W = op.i[2];
   if (op.i[3] <= CUT_MAX_CUTN && op.i[4] <= 32768) {  // row-per-block gather with shared per-cutout row tables
-    CGD_CUDA(launch_pdl(cutouts_bwd_rows_kernel, dim3((unsigned)(B * H * ceil_div(W, CUT_BWD_THREADS))), dim3(CUT_BWD_THREADS), 0, st, (const __half*)op.p[0], (const int*)op.p[1], (float*)op.p[2],
+    CGD_CUDA(launch_pdl(acc ? cutouts_bwd_rows_kernel<true> : cutouts_bwd_rows_kernel<false>, dim3((unsigned)(B * H * ceil_div(W, CUT_BWD_THREADS))),
+                        dim3(CUT_BWD_THREADS), 0, st, (const __half*)op.p[0], (const int*)op.p[1], (float*)op.p[2],
                         (int)B, (int)H, (int)W, (int)op.i[3], (int)op.i[4], (int)op.i[5], (int)op.i[6], make_float3(op.f[3], op.f[4], op.f[5]), op.f[6]));
     CGD_LAUNCH_CHECK();
     return 0;
   }
-  CGD_CUDA(launch_pdl(cutouts_bwd_kernel, dim3(gw_blocks(B * 3 * H * W)), dim3(256), 0, st, (const __half*)op.p[0], (const int*)op.p[1], (float*)op.p[2], (int)B, (int)H,
-                                                              (int)W, (int)op.i[3], (int)op.i[4], (int)op.i[5], (int)op.i[6],
-                                                              make_float3(op.f[3], op.f[4], op.f[5]), op.f[6]));
+  CGD_CUDA(launch_pdl(acc ? cutouts_bwd_kernel<true> : cutouts_bwd_kernel<false>, dim3(gw_blocks(B * 3 * H * W)), dim3(256), 0, st, (const __half*)op.p[0],
+                      (const int*)op.p[1], (float*)op.p[2], (int)B, (int)H, (int)W, (int)op.i[3], (int)op.i[4], (int)op.i[5], (int)op.i[6],
+                      make_float3(op.f[3], op.f[4], op.f[5]), op.f[6]));
   CGD_LAUNCH_CHECK();
   return 0;
 }

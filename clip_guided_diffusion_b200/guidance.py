@@ -9,6 +9,8 @@ Surfaces kept (SURVEY.md 8b): ``cond_fn(x, t, out, y=None)``, ``MakeCutouts``, `
 """
 from __future__ import annotations
 
+import itertools
+
 import numpy as np
 import torch as th
 
@@ -160,8 +162,30 @@ class EngineModel:
         return collections.namedtuple("IncompatibleKeys", "missing_keys unexpected_keys")(missing, unexpected)
 
 
+def _as_list(v):
+    """a list or tuple (one item per CLIP tower) -> list(v); anything else is one item -> [v]"""
+    return list(v) if isinstance(v, (list, tuple)) else [v]
+
+
+class _Tower:
+    """one CLIP tower of the engine: its config, the windows it cuts, its targets, one tower instance per cutout count"""
+
+    def __init__(self, cfg, coords, targets, vit, tag):
+        self.cfg, self.coords, self.targets, self.vit, self.tag = cfg, coords, targets, vit, tag
+        self.vits = {}
+
+    def sfx(self, count_sfx=""):
+        """range-mark suffix: the cutout count's ("@c", "" for the default count), then the tower's ("", "#1", "#2", ...)"""
+        return count_sfx + self.tag
+
+
 class GuidedStepB200:
-    """Engine for one (local batch, H, W, cutn, CLIP tower) configuration on one GPU."""
+    """Engine for one (local batch, H, W, cutn, CLIP towers) configuration on one GPU.
+
+    ``vit_cfg`` / ``vit_sd``: one CLIP visual tower, or equal-length sequences of them (an ensemble).  Every tower cuts its own windows at
+    its own resolution and gets its own targets; their CLIP losses are summed (the reference's CLIP block once per tower) and share the
+    prompt weights.  The towers run one after another inside the step; the first stores its cutout gradient, the others add theirs
+    (CUTOUTS_BWD flags 2), in tower order."""
 
     def __init__(self, unet_cfg: UNetConfig, unet_sd: dict, vit_cfg: ViTConfig = None, vit_sd: dict = None, *, batch: int,
                  height: int = None, width: int = None, num_cutouts: int = 16, max_prompts: int = 1, clip_guidance_scale=1000.0,
@@ -176,6 +200,14 @@ class GuidedStepB200:
         self.H = height or unet_cfg.image_size
         self.W = width or unet_cfg.image_size
         self.cutn = num_cutouts if vit_cfg is not None else 0
+        cfgs = _as_list(vit_cfg) if vit_cfg is not None else []
+        sds = _as_list(vit_sd) if vit_cfg is not None else []
+        if vit_cfg is not None and (not cfgs or len(sds) != len(cfgs)):
+            raise ValueError(f"vit_cfg / vit_sd: one CLIP tower or equal-length non-empty sequences (got {len(cfgs)} configs, {len(sds)} state_dicts)")
+        if len(cfgs) > 1 and (use_augs or cutout_resize != "pool"):
+            raise NotImplementedError("several CLIP towers run with the reference's adaptive_avg_pool2d cutouts and no augmentations "
+                                      "(use_augs and cutout_resize='lanczos3' need per-tower parameters)")
+        self.T = len(cfgs)
         self.P = max_prompts
         self.scales = dict(cgs=float(clip_guidance_scale), tv=float(tv_scale), rng=float(range_scale), sat=float(sat_scale))
         self.use_magnitude = bool(use_magnitude)
@@ -204,7 +236,10 @@ class GuidedStepB200:
         self.vit = None
         self.lpips = None
         self.use_augs = False
+        self.towers = []
+        self.loss_towers = None
         if vit_cfg is not None:
+            vit_cfg, vit_sd = cfgs[0], sds[0]
             cutn, cs, ps, kp, D = self.cutn, vit_cfg.input_resolution, vit_cfg.patch_size, vit_cfg.kpad, vit_cfg.output_dim
             self.vit_cfg = vit_cfg
             self.coords = p.new(cutn * 3, "i32", "cutout_coords")
@@ -219,6 +254,8 @@ class GuidedStepB200:
             # further cutout counts of the same engine (progressive_cutout, cgd/cgd.py:167-175): own activations and op ranges
             # ("...@c" marks), shared packed weights; the default count keeps the un-suffixed marks
             self.vits = {cutn: self.vit}
+            self.towers.append(_Tower(vit_cfg, self.coords, self.targets, self.vit, ""))
+            self.towers[0].vits = self.vits
             # cutout resampling: "pool" = adaptive_avg_pool2d like the reference's MakeCutouts (cgd/modules.py:63); "lanczos3" =
             # the vendored ResizeRight resampler north_star names (cgd/ResizeRight/resize_right.py, host tables in resize_right.py)
             if cutout_resize not in ("pool", "lanczos3"):
@@ -245,12 +282,28 @@ class GuidedStepB200:
                 self.rr_w = p.new(cutn * cs * T_MAX, "f", "rr_weights")
                 self.rr_taps = p.new(cutn, "i32", "rr_taps")
                 self.rr_inv = p.new(cutn * H * 2, "i32", "rr_inverse")
-            for c in sorted(set(int(v) for v in cutn_variants) - {cutn}):
+            variants = sorted(set(int(v) for v in cutn_variants) - {cutn})
+            for c in variants:
                 if not 0 < c < cutn:
                     raise ValueError(f"cutn_variants must lie in (0, {cutn}), got {c}")
                 self.vits[c] = Tower(vit_cfg, vit_sd, n_images=c * B, device=device, plan=p, parts=vit_streams, suffix=f"@{c}", share=self.vit)
-            for c in sorted(self.vits, key=lambda v: v == cutn):  # the default count last: its ranges end at "guide"
-                sfx, vt = ("" if c == cutn else f"@{c}"), self.vits[c]
+            # towers 1.. of an ensemble: own windows, targets and activations; range marks suffixed "#m" (tower 0 keeps the plain ones)
+            for m, (cfg_m, sd_m) in enumerate(zip(cfgs[1:], sds[1:]), start=1):
+                Tower_m = RNB200 if isinstance(cfg_m, RNConfig) else ViTB200
+                tw = _Tower(cfg_m, p.new(cutn * 3, "i32", f"cutout_coords#{m}"), p.new(self.P * cfg_m.output_dim, "f", f"target_embeds#{m}"),
+                            None, f"#{m}")
+                tw.vit = Tower_m(cfg_m, sd_m, n_images=cutn * B, device=device, plan=p, parts=vit_streams, suffix=tw.tag)
+                tw.vits[cutn] = tw.vit
+                for c in variants:
+                    tw.vits[c] = Tower_m(cfg_m, sd_m, n_images=c * B, device=device, plan=p, parts=vit_streams, suffix=f"@{c}" + tw.tag, share=tw.vit)
+                self.towers.append(tw)
+            # clip terms of towers 1..: [T - 1, B] (tower 0's stays in `loss`); SPHERICAL stores them, nothing needs zeroing
+            self.loss_towers = p.new((self.T - 1) * B, "f", "losses_towers") if self.T > 1 else None
+            # per cutout count (the default count last: its ranges end at "guide"), then per tower in tower order
+            for c, (m, tw) in itertools.product(sorted(self.vits, key=lambda v: v == cutn), enumerate(self.towers)):
+                sfx, vt = tw.sfx("" if c == cutn else f"@{c}"), tw.vits[c]
+                cs, ps, kp, D = tw.cfg.input_resolution, tw.cfg.patch_size, tw.cfg.kpad, tw.cfg.output_dim
+                coords_m, loss_m = (tw.coords, 0), ((self.loss, 0) if m == 0 else (self.loss_towers, (m - 1) * B))
                 p.mark("cut_fwd" + sfx)
                 if cutout_resize == "lanczos3":
                     p.emit("CUTOUTS_RR_FWD", i=[B, H, W, c, cs, ps, kp], f=[*CLIP_MEAN, *CLIP_STD],
@@ -261,11 +314,11 @@ class GuidedStepB200:
                            p=[(self.x_inb, 0), (self.coords, 0), (vt.patches, 0), (self.aug_prm, 0), (self.aug_noise, 0)],
                            tag="make_cutouts(use_augs)+normalize")
                 else:
-                    p.emit("CUTOUTS_FWD", i=[B, H, W, c, cs, ps, kp], f=[*CLIP_MEAN, *CLIP_STD], p=[(self.x_inb, 0), (self.coords, 0), (vt.patches, 0)],
+                    p.emit("CUTOUTS_FWD", i=[B, H, W, c, cs, ps, kp], f=[*CLIP_MEAN, *CLIP_STD], p=[(self.x_inb, 0), coords_m, (vt.patches, 0)],
                            tag="make_cutouts+normalize")
                 p.mark("sph" + sfx)
                 p.emit("SPHERICAL", i=[c, B, self.P, D], f=[self.scales["cgs"], self.vit_grad_scale],
-                       p=[(vt.embeds, 0), (self.targets, 0), (self.weights, 0), (vt.d_embeds, 0), (self.loss, 0)], tag="spherical_dist_loss")
+                       p=[(vt.embeds, 0), (tw.targets, 0), (self.weights, 0), (vt.d_embeds, 0), loss_m], tag="spherical_dist_loss")
                 p.mark("cut_bwd" + sfx)
                 if cutout_resize == "lanczos3":
                     p.emit("CUTOUTS_RR_BWD", i=[B, H, W, c, cs, ps, kp, H], f=[0, 0, 0, *CLIP_STD, 1.0 / self.vit_grad_scale],
@@ -276,8 +329,9 @@ class GuidedStepB200:
                     p.emit("CUTOUTS_AUG_BWD", i=[B, H, W, c, cs, ps, kp], f=[0, 0, 0, *CLIP_STD, 1.0 / self.vit_grad_scale],
                            p=[(vt.d_patches, 0), (self.coords, 0), (self.g_clip, 0), (self.aug_prm, 0)], tag="d_make_cutouts(use_augs)")
                 else:
-                    p.emit("CUTOUTS_BWD", i=[B, H, W, c, cs, ps, kp], f=[0, 0, 0, *CLIP_STD, 1.0 / self.vit_grad_scale],
-                           p=[(vt.d_patches, 0), (self.coords, 0), (self.g_clip, 0)], tag="d_make_cutouts")
+                    # tower 0 stores the x_in gradient, towers 1.. add theirs (flags 2) in tower order: a deterministic sum
+                    p.emit("CUTOUTS_BWD", flags=0 if m == 0 else 2, i=[B, H, W, c, cs, ps, kp], f=[0, 0, 0, *CLIP_STD, 1.0 / self.vit_grad_scale],
+                           p=[(vt.d_patches, 0), coords_m, (self.g_clip, 0)], tag="d_make_cutouts")
                 p.mark("cut_end" + sfx)
             if lpips_sd is not None and init_scale != 0:
                 from .lpips import LpipsB200
@@ -320,7 +374,7 @@ class GuidedStepB200:
         self.model = EngineModel(self)
         self.shape = (B, 3, H, W)
         # pinned staging for the per-step host->device refresh
-        self._n_stage = SC["COUNT"] * 4 + self.cutn * 3 * 4 + B * 4 + B * 8 + self.cutn * 20 * 4
+        self._n_stage = SC["COUNT"] * 4 + self.cutn * 3 * 4 + B * 4 + B * 8 + self.cutn * 20 * 4 + max(self.T - 1, 0) * self.cutn * 3 * 4
         # The host runs ahead of the GPU (a step is ~1 ms of host work and ~10 ms of device work, and nothing synchronises between
         # saved frames), so the async copies of step k may still be queued when the host stages step k+1: the pinned buffers are a
         # ring of STAGE_SLOTS slots, each guarded by the event recorded after its copies were enqueued.
@@ -330,7 +384,7 @@ class GuidedStepB200:
         self._stage_i = 0
         self._rr_ring = None
         self._graphs = {}
-        self._side_streams = [th.cuda.Stream(device=self.device) for _ in range((self.vit.parts if self.vit is not None else 1) - 1)] \
+        self._side_streams = [th.cuda.Stream(device=self.device) for _ in range(max((tw.vit.parts for tw in self.towers), default=1) - 1)] \
             if self.device.type == "cuda" else []
         self._last_out = None
         self._fwd_valid = False
@@ -350,16 +404,22 @@ class GuidedStepB200:
             raise RuntimeError("engine built without the LPIPS loss (pass lpips_sd= and init_scale != 0)")
         self.lpips.set_init_image(init, runner)
 
-    def set_targets(self, target_embeds: th.Tensor, weights: th.Tensor):
-        """target_embeds [P, D] (un-normalised is fine: the loss normalises, cgd/losses.py:12-13); weights already divided by
-        their |sum| like cgd/cgd.py:102-105."""
-        P = target_embeds.shape[0]
-        if P != self.P:
-            raise ValueError(f"engine was built for {self.P} prompt(s), got {P}")
-        if self.B > 1 and P > 1:
+    def set_targets(self, target_embeds, weights: th.Tensor):
+        """target_embeds [P, D] (un-normalised is fine: the loss normalises, cgd/losses.py:12-13), or one [P, D_m] per tower of an
+        ensemble; weights [P] (shared by the towers) already divided by their |sum| like cgd/cgd.py:102-105."""
+        per = _as_list(target_embeds)
+        if self.T > 1 and isinstance(target_embeds, th.Tensor):
+            raise ValueError(f"engine built with {self.T} CLIP towers: target_embeds must be a sequence of {self.T} [P, D_m] tensors")
+        if len(per) != self.T:
+            raise ValueError(f"engine built with {self.T} CLIP tower(s), got {len(per)} target tensors")
+        for tw, te in zip(self.towers, per):
+            if tuple(te.shape) != (self.P, tw.cfg.output_dim):
+                raise ValueError(f"engine was built for {self.P} prompt(s) of width {tw.cfg.output_dim}, got {tuple(te.shape)}")
+        if self.B > 1 and self.P > 1:
             raise RuntimeError("the reference's spherical-loss broadcast is only defined for batch 1 or a single prompt (quirk B1)")
-        self.v(self.targets, (P, self.vit_cfg.output_dim)).copy_(target_embeds.detach().float())
-        self.v(self.weights, (P,)).copy_(weights.detach().float())
+        for tw, te in zip(self.towers, per):
+            self.v(tw.targets, (self.P, tw.cfg.output_dim)).copy_(te.detach().float())
+        self.v(self.weights, (self.P,)).copy_(weights.detach().float())
 
     # ------------------------------------------------------------------ RNG (torch generators: seed parity, SURVEY 8e)
     def local_rows(self, t: th.Tensor) -> th.Tensor:
@@ -427,18 +487,22 @@ class GuidedStepB200:
             sc = diffusion.scalar_table(self._cur_t, fac_index)
             self._push_scalars(sc)
             self.plan.run_range("pmv", "cond")
-        cutn = len(coords)
-        sfx = self._sfx(cutn)
-        self.v(self.coords, (self.cutn, 3))[:cutn].copy_(th.tensor(coords, dtype=th.int32), non_blocking=True)
-        self._stage_resize_tables(coords)
+        per = self._per_tower(coords)
+        cutn = len(per[0])
+        csfx = self._sfx(cutn)
+        for tw, cm in zip(self.towers, per):
+            self.v(tw.coords, (self.cutn, 3))[:cutn].copy_(th.tensor(cm, dtype=th.int32), non_blocking=True)
+        self._stage_resize_tables(per[0])
         if self.use_augs:
-            self._stage_augs(coords)
-        self.plan.run_range("cut_fwd" + sfx, "sph" + sfx)
-        self._run_vit("fwd", None, cutn)
-        self.plan.run_range("sph" + sfx, "cut_bwd" + sfx)
-        self._run_vit("bwd", None, cutn)
-        for a, b in (("cut_bwd" + sfx, "cut_end" + sfx),) + ((("lpips", "lpips_end"),) if self.lpips is not None else ()) + (
-                ("guide", "final"), ("unet_bwd", "unet_end")):
+            self._stage_augs(per[0])
+        for m, tw in enumerate(self.towers):
+            sfx = tw.sfx(csfx)
+            self.plan.run_range("cut_fwd" + sfx, "sph" + sfx)
+            self._run_vit("fwd", None, cutn, m)
+            self.plan.run_range("sph" + sfx, "cut_bwd" + sfx)
+            self._run_vit("bwd", None, cutn, m)
+            self.plan.run_range("cut_bwd" + sfx, "cut_end" + sfx)
+        for a, b in ((("lpips", "lpips_end"),) if self.lpips is not None else ()) + (("guide", "final"), ("unet_bwd", "unet_end")):
             self.plan.run_range(a, b)
         self._run_final(self.plan.run_range)
         return self.img(self.g)
@@ -478,16 +542,29 @@ class GuidedStepB200:
             raise ValueError(f"engine built for cutout counts {sorted(self.vits)}, got {cutn}")
         return f"@{cutn}"
 
+    def _per_tower(self, coords):
+        """a step's cutout windows -> one window list per tower: one tower takes a flat window list, an ensemble a sequence of
+        them (the same count each); no windows at all (an unguided step) -> empty lists"""
+        if self.T <= 1 or not len(coords):
+            return [list(coords)] * max(self.T, 1)
+        per = [list(c) for c in coords]
+        if len(per) != self.T or len({len(c) for c in per}) != 1:
+            raise ValueError(f"engine built with {self.T} CLIP towers: expected {self.T} window lists of one length, got "
+                             f"{[len(c) for c in per]}")
+        return per
+
     def _run_all(self, mode, runner=None, cutn=None, part=None):
         pr = runner or self.plan.run_range
-        sfx = self._sfx(cutn)
+        csfx = self._sfx(cutn)
         pr("unet_emb", "unet_bwd")
         pr("pmv", "cond")
-        pr("cut_fwd" + sfx, "sph" + sfx)
-        self._run_vit("fwd", pr, cutn)
-        pr("sph" + sfx, "cut_bwd" + sfx)
-        self._run_vit("bwd", pr, cutn)
-        pr("cut_bwd" + sfx, "cut_end" + sfx)
+        for m, tw in enumerate(self.towers):  # one tower after another: cutouts -> fwd -> loss -> bwd -> cutout gradient
+            sfx = tw.sfx(csfx)
+            pr("cut_fwd" + sfx, "sph" + sfx)
+            self._run_vit("fwd", pr, cutn, m)
+            pr("sph" + sfx, "cut_bwd" + sfx)
+            self._run_vit("bwd", pr, cutn, m)
+            pr("cut_bwd" + sfx, "cut_end" + sfx)
         if self.lpips is not None:
             pr("lpips", "lpips_end")
         pr("guide", "final")
@@ -504,11 +581,11 @@ class GuidedStepB200:
         else:
             pr("upd_ddim_g", "upd_ddim")
 
-    def _run_vit(self, which, pr=None, cutn=None):
-        """CLIP forward / backward: one op range, or one per batch slice on parallel streams (fork / join around the current
-        stream; inside CUDA-graph capture this becomes parallel branches of the graph)."""
+    def _run_vit(self, which, pr=None, cutn=None, tower=0):
+        """CLIP forward / backward of one tower: one op range, or one per batch slice on parallel streams (fork / join around the
+        current stream; inside CUDA-graph capture this becomes parallel branches of the graph)."""
         pr = pr or self.plan.run_range
-        ranges = self.vits[self.cutn if cutn is None else cutn].part_ranges(which)
+        ranges = self.towers[tower].vits[self.cutn if cutn is None else cutn].part_ranges(which)
         if len(ranges) == 1 or not self._side_streams or pr != self.plan.run_range:
             for a, b in ranges:
                 pr(a, b)
@@ -523,8 +600,10 @@ class GuidedStepB200:
 
     def launches_per_step(self, mode="ddim") -> int:
         m = self.plan.marks
-        segs = [("unet_emb", "unet_bwd"), ("pmv", "cond"), ("cut_fwd", "sph"), ("vit_fwd", "vit_bwd"), ("sph", "cut_bwd"), ("vit_bwd", "vit_end"),
-                ("cut_bwd", "cut_end")] + ([("lpips", "lpips_end")] if self.lpips is not None else []) + [
+        segs = [("unet_emb", "unet_bwd"), ("pmv", "cond")] + [
+                (a + t, b + t) for t in (tw.tag for tw in self.towers) for a, b in (
+                    ("cut_fwd", "sph"), ("vit_fwd", "vit_bwd"), ("sph", "cut_bwd"), ("vit_bwd", "vit_end"), ("cut_bwd", "cut_end"))] + (
+                [("lpips", "lpips_end")] if self.lpips is not None else []) + [
                 ("guide", "final"), ("unet_bwd", "unet_end"), ("final", "upd_anc_g"),
                 ("upd_anc_g", "upd_anc") if mode == "ancestral" else ("upd_ddim_g", "upd_ddim")]  # "mag" lies inside (final, upd_anc_g)
         return sum(self.plan.num_launches(m[a], m[b] - m[a]) for a, b in segs)
@@ -568,13 +647,15 @@ class GuidedStepB200:
         self.v(self.unet.t_in).view(th.uint8).copy_(st[o:o + n], non_blocking=True)
         o += n
         self.h2d_bytes += SC["COUNT"] * 4 + self.B * 4
+        per = self._per_tower(coords) if self.cutn else []
         if self.cutn:
-            for ox, oy, size in coords:  # windows may be clipped at the border (quirk B3) but not empty
+            for ox, oy, size in itertools.chain(*per):  # windows may be clipped at the border (quirk B3) but not empty
                 if not (0 <= ox < self.W and 0 <= oy < self.H and size > 0):
                     raise RuntimeError(f"cutout window (x={ox}, y={oy}, size={size}) lies outside the {self.H}x{self.W} image: the reference's "
                                        "adaptive_avg_pool2d raises on the empty crop (non-square images, cgd/modules.py:52,61)")
-            n = len(coords) * 12
-        if self.cutn and len(coords):
+            n = len(per[0]) * 12
+        if self.cutn and len(per[0]):
+            coords = per[0]
             st[o:o + n].view(th.int32).copy_(th.tensor(coords, dtype=th.int32).view(-1))
             self.v(self.coords).view(th.uint8)[:n].copy_(st[o:o + n], non_blocking=True)
             self.h2d_bytes += n
@@ -582,6 +663,12 @@ class GuidedStepB200:
             self._stage_resize_tables(coords, k)
             if getattr(self, "use_augs", False):
                 self._stage_augs(coords, st, o)
+            o += self.cutn * 20 * 4
+            for tw, cm in zip(self.towers[1:], per[1:]):  # the other towers' windows follow the use_augs region
+                st[o:o + n].view(th.int32).copy_(th.tensor(cm, dtype=th.int32).view(-1))
+                self.v(tw.coords).view(th.uint8)[:n].copy_(st[o:o + n], non_blocking=True)
+                self.h2d_bytes += n
+                o += self.cutn * 12
         self._stage_release(k)
 
     def _stage_augs(self, coords, st=None, o=0):
@@ -648,7 +735,7 @@ class GuidedStepB200:
         xin = self.img(self.unet.x_in)
         if img.data_ptr() != xin.data_ptr():
             xin.copy_(img, non_blocking=True)
-        self.replay(mode, len(coords) if (self.cutn and guided) else None, guided=guided)
+        self.replay(mode, len(self._per_tower(coords)[0]) if (self.cutn and guided) else None, guided=guided)
         return {"sample": self.img(self.sample).clone(), "pred_xstart": self.img(self.x0).clone()}
 
     def _run_unguided(self, mode, pr=None):
@@ -711,7 +798,9 @@ class GuidedStepB200:
     def losses(self) -> dict:
         """per-image loss terms of the last step (device->host sync; logging only, like tqdm.write at cgd/cgd.py:234-236)"""
         l = self.v(self.loss, (4, self.B)).cpu()
-        d = {"clip": l[0], "tv": l[1], "range": l[2], "sat": l[3]}
+        per = l[0:1] if self.loss_towers is None else th.cat([l[0:1], self.v(self.loss_towers, (self.T - 1, self.B)).cpu()])
+        # "clip": the sum over the towers, in tower order; "clip_per_tower": [T, B]
+        d = {"clip": per.sum(0), "clip_per_tower": per, "tv": l[1], "range": l[2], "sat": l[3]}
         if self.lpips is not None:
             d["init"] = self.lpips.loss_value().cpu() * self.lpips.init_scale
         return d
@@ -723,8 +812,15 @@ class CondFnB200:
 
     with_grad = True
 
-    def __init__(self, engine: GuidedStepB200, diffusion, make_cutouts: MakeCutouts, *, cached_cutouts=False, reduce_clip=False,
+    def __init__(self, engine: GuidedStepB200, diffusion, make_cutouts, *, cached_cutouts=False, reduce_clip=False,
                  progressive_cutout=False):
+        """``make_cutouts``: one ``MakeCutouts``, or one per CLIP tower of an ensemble engine (in tower order, the same count each)"""
+        self.cutouts = _as_list(make_cutouts)
+        if not self.cutouts or len({mk.cutn for mk in self.cutouts}) != 1:
+            raise ValueError("make_cutouts: one MakeCutouts or a non-empty sequence of them with the same num_cutouts")
+        if engine.cutn and len(self.cutouts) != getattr(engine, "T", 1):  # (duck-typed engines without towers count as one)
+            raise ValueError(f"engine built with {engine.T} CLIP tower(s), got {len(self.cutouts)} MakeCutouts")
+        make_cutouts = self.cutouts[0]
         self.engine, self.diffusion, self.make_cutouts = engine, diffusion, make_cutouts
         self.cached_cutouts, self.reduce_clip, self.progressive_cutout = cached_cutouts, reduce_clip, progressive_cutout
         self.current_timestep = diffusion.num_timesteps - 1  # cgd/cgd.py:265
@@ -766,7 +862,11 @@ class CondFnB200:
         self.current_timestep -= 1
 
     def next_coords(self, H, W):
-        return self.make_cutouts.coords_for(H, W, use_cache=self.cached_cutouts, num_cutouts_override=self.current_cutn())
+        """this step's windows: a flat list for one tower; with several, one list per tower, drawn in tower order (each tower
+        with its own min_size = min(H, W, cut_size))"""
+        n = self.current_cutn()
+        per = [mk.coords_for(H, W, use_cache=self.cached_cutouts, num_cutouts_override=n) for mk in self.cutouts]
+        return per[0] if len(per) == 1 else per
 
     def __call__(self, x, t, out, y=None):
         eng = self.engine

@@ -133,7 +133,9 @@ enum {
    * i0 B i1 H i2 W i3 cutn i4 cut_size i5 patch i6 Kpad ; f0..2 mean f3..5 std */
   /* (CUTOUTS_FWD flags 1: p2 is fp32 instead of fp16 -- the stand-alone MakeCutouts surface returns fp32 like the reference) */
   CGD_OP_CUTOUTS_FWD = 21,
-  /* gather-style backward (no atomics): p0 dpatches(h) p1 coords p2 dx_in(f NCHW) ; i as fwd ; f3..5 std ; f6 scale */
+  /* gather-style backward (no atomics): p0 dpatches(h) p1 coords p2 dx_in(f NCHW) ; i as fwd ; f3..5 std ; f6 scale
+   * flags 0 = store into dx_in ; 2 = add to it (several CLIP towers: the first stores, the others add in launch order, so the sum is
+   * deterministic and bitwise old + the flags-0 result) ; any other flags are rejected */
   CGD_OP_CUTOUTS_BWD = 22,
   /* spherical_dist_loss + prompt weights + cutout mean, with analytic d/d(embed) (cgd/losses.py:10-14,
    * cgd/cgd.py:196-200,204; SURVEY K17).  p0 emb(f [cutn*B, D]) p1 targets(f [P,D]) p2 weights(f [P])
