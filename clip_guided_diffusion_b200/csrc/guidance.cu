@@ -611,8 +611,9 @@ __global__ void guide_grad_kernel(const float* __restrict__ xin, const float* __
 }
 // Dynamic seed scaling (flags & 1 of GUIDE_GRAD): d L / d eps = -sqrt(1/abar - 1) * d L / d pred_xstart spans many orders of
 // magnitude over a chain (the factor alone runs from 0.01 to 157) and is the seed of an fp16 backward.  Per image, the seed is
-// multiplied by the power of two that puts its largest element at [2048, 4096) (exact in fp16, 16x headroom for growth inside
-// the backward, 2^-24 / 4096 of dynamic range below), and FINAL_GRAD divides the input gradient by the same factor.
+// multiplied by the power of two that puts its largest element m in (2048, 4096] (scale = 2^floor(log2(4096 / m)): m = 2048 and
+// m = 4096 both land on 4096; exact in fp16, 16x headroom for growth inside the backward, 2^-24 / 4096 of dynamic range below; the
+// exponent is clamped to [-60, 60]), and FINAL_GRAD divides the input gradient by the same factor.
 // dyn layout: [B] max |seed| (float bits, reset to 0 by FINAL_GRAD) | [B] scale.
 __global__ void seed_quant_kernel(const float* __restrict__ seed_f32, float* __restrict__ dyn, __half* __restrict__ seed, int B, int64_t HW,
                                   int64_t ld) {

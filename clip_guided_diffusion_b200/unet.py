@@ -88,6 +88,47 @@ def topology(cfg: UNetConfig):
     return blocks_in, mid_ch, blocks_out
 
 
+def emit_emb_layers(p: Plan, cfg: UNetConfig, B: int, emb, weight):
+    """The prelude's scale-shift vectors: every ResBlock's emb_layers Linear (e = Linear(SiLU(emb)) -> [B, 2*Cout] fp32,
+    x-independent: no backward), all evaluated by ONE weight-streaming launch: ~30 launches of 8 MB fp32 each (0.43 ms per step)
+    become one pass over the concatenated fp16 weights (the reference's emb_layers are fp16 too: convert_to_fp16 covers the
+    ResBlocks, cgd/script_util.py:322-323), scattered into each ResBlock's own [B, 2*Cout] buffer by a per-column table.
+
+    `emb` is the [B, 4*model_channels] fp32 embedding buffer, `weight(key)` returns a state-dict tensor (fp32, CPU).  Returns
+    topology(cfg)'s (blocks_in, mid_ch, blocks_out) with each block's vector in b["e"] (and b["e_up"] for the upsampling ResBlock
+    of an output level), the two middle-block vectors, and the jobs [(state-dict prefix, 2*Cout, output Buf)] in table order."""
+    blocks_in, mid_ch, blocks_out = topology(cfg)
+    jobs = []
+
+    def prepare(prefix, cout):
+        e = p.new(B * 2 * cout, "f", prefix + ".emb_layers.1_e")
+        jobs.append((prefix + ".emb_layers.1", 2 * cout, e))
+        return e
+
+    for b in blocks_in:
+        b["e"] = prepare(b["prefix"] + ".0", b["cout"])
+    mid_e = [prepare("middle_block.0", mid_ch), prepare("middle_block.2", mid_ch)]
+    for b in blocks_out:
+        b["e"] = prepare(b["prefix"] + ".0", b["cout"])
+        if b["up"]:
+            b["e_up"] = prepare(b["prefix"] + (".2" if b["attn"] else ".1"), b["cout"])
+
+    ted = 4 * cfg.model_channels
+    W = th.cat([weight(k + ".weight") for k, _, _ in jobs], dim=0)
+    bias = th.cat([weight(k + ".bias") for k, _, _ in jobs], dim=0)
+    base = jobs[0][2].off
+    tab = []
+    for _, cout2, e in jobs:
+        assert (e.off - base) % 4 == 0
+        off = (e.off - base) // 4
+        tab += [[off + c, cout2] for c in range(cout2)]
+    n_total = W.shape[0]
+    p.emit("LINEAR_SMALL", flags=1 | 16, i=[B, ted, n_total, ted, n_total],
+           p=[(emb, 0), (p.const(W, "h", "emb_layers.W"), 0), (p.const(bias, "f", "emb_layers.b"), 0), (jobs[0][2], 0),
+              (p.const(th.tensor(tab, dtype=th.int32), "i32", "emb_layers.scatter"), 0)], tag="emb_layers (all ResBlocks)")
+    return blocks_in, mid_ch, blocks_out, mid_e, jobs
+
+
 IN_PAD = 64  # image channels are zero-padded to one 64-channel K slice for the stem conv / head dgrad
 
 
@@ -129,32 +170,6 @@ class UNetB200:
 
     def _conv_w(self, prefix, need_bwd=True, cin_pad=None) -> ConvW:
         return pack_conv(self.plan, self._w(prefix + ".weight"), self._w(prefix + ".bias"), need_bwd=need_bwd, cin_pad=cin_pad, name=prefix)
-
-    def _resblock_prepare(self, prefix, cout):
-        """Register one ResBlock's emb_layers Linear (e = Linear(SiLU(emb)) -> [B, 2*Cout] fp32, x-independent: no backward).
-        All of them are evaluated by ONE weight-streaming launch in the prelude (`_emit_emb_layers`): ~30 launches of 8 MB fp32
-        each (0.43 ms per step) become one pass over the concatenated fp16 weights (the reference's emb_layers are fp16 too:
-        convert_to_fp16 covers the ResBlocks, cgd/script_util.py:322-323)."""
-        cout2 = 2 * cout
-        e = self.plan.new(self.B * cout2, "f", prefix + ".emb_layers.1_e")
-        self._emb_jobs.append((prefix + ".emb_layers.1", cout2, e))
-        return e
-
-    def _emit_emb_layers(self):
-        p = self.plan
-        ted = 4 * self.cfg.model_channels
-        W = th.cat([self._w(k + ".weight") for k, _, _ in self._emb_jobs], dim=0)
-        b = th.cat([self._w(k + ".bias") for k, _, _ in self._emb_jobs], dim=0)
-        base = self._emb_jobs[0][2].off
-        tab = []
-        for _, cout2, e in self._emb_jobs:
-            assert (e.off - base) % 4 == 0
-            off = (e.off - base) // 4
-            tab += [[off + c, cout2] for c in range(cout2)]
-        n_total = W.shape[0]
-        p.emit("LINEAR_SMALL", flags=1 | 16, i=[self.B, ted, n_total, ted, n_total],
-               p=[(self.emb, 0), (p.const(W, "h", "emb_layers.W"), 0), (p.const(b, "f", "emb_layers.b"), 0), (self._emb_jobs[0][2], 0),
-                  (p.const(th.tensor(tab, dtype=th.int32), "i32", "emb_layers.scatter"), 0)], tag="emb_layers (all ResBlocks)")
 
     def _resblock(self, x: Act, prefix: str, cout: int, e_buf, up=False, down=False, out: Act = None) -> Act:
         p = self.plan
@@ -207,18 +222,8 @@ class UNetB200:
         if cfg.class_cond:
             p.emit("LABEL_ADD", i=[B, ted], p=[(self.emb, 0), (self._const("label_emb.weight"), 0), (self.y_in, 0)], tag="label_emb")
 
-        blocks_in, mid_ch, blocks_out = topology(cfg)
         # scale-shift vectors (prelude ops must precede the trunk)
-        self._emb_jobs = []
-        for b in blocks_in:
-            b["e"] = self._resblock_prepare(b["prefix"] + ".0", b["cout"])
-        mid_e = [self._resblock_prepare("middle_block.0", mid_ch), self._resblock_prepare("middle_block.2", mid_ch)]
-        for b in blocks_out:
-            b["e"] = self._resblock_prepare(b["prefix"] + ".0", b["cout"])
-            if b["up"]:
-                b["e_up"] = self._resblock_prepare(b["prefix"] + (".2" if b["attn"] else ".1"), b["cout"])
-
-        self._emit_emb_layers()
+        blocks_in, mid_ch, blocks_out, mid_e, _ = emit_emb_layers(p, cfg, B, self.emb, self._w)
 
         # ---- forward trunk
         p.mark("unet_fwd")
