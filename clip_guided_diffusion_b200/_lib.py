@@ -75,3 +75,18 @@ def check(rc: int, what: str = ""):
     if rc != 0:
         msg = load().cgd_last_error().decode("utf-8", "replace")
         raise CgdError(f"{what + ': ' if what else ''}libcgd_b200 error {rc}: {msg}")
+
+
+def run_op(code: str, *, flags=0, i=(), f=(), p=(), what=None):
+    """one op outside a plan, on the current CUDA stream: `i` ints, `f` floats, `p` tensors (their data pointers); raises CgdError
+    (prefixed `what`, default the op name) when the library refuses it"""
+    import torch as th
+    op = CgdOp()
+    op.code, op.flags = OP[code], flags
+    for j, v in enumerate(i):
+        op.i[j] = int(v)
+    for j, v in enumerate(f):
+        op.f[j] = float(v)
+    for j, t in enumerate(p):
+        op.p[j] = t.data_ptr()
+    check(load().cgd_run_op(ctypes.byref(op), ctypes.c_void_p(th.cuda.current_stream().cuda_stream)), what or code.lower())

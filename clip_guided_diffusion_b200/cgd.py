@@ -36,7 +36,7 @@ from pathlib import Path
 import torch as th
 
 from . import gaussian_diffusion as gd
-from .guidance import CondFnB200, GuidedStepB200, MakeCutouts
+from .guidance import CondFnB200, GuidedStepB200, MakeCutouts, check_tower_options
 from .image_prompt import ImagePromptEncoder, check_local
 from .text import TextB200, text_config_from_state_dict
 from .tokenizer import find_vocab, load_tokenizer, tokenize  # noqa: F401 (tokenize: public, like clip.tokenize)
@@ -280,10 +280,7 @@ def clip_guided_diffusion(
     _require_cuda(device)
     names, clip_sds = _tower_list(clip_model_name, clip_state_dict)
     T = len(names)
-    if T > 1 and use_augs:
-        raise NotImplementedError("use_augs with several CLIP towers (the augmentation parameters are drawn for one tower's cutouts)")
-    if T > 1 and cutout_resize == "lanczos3":
-        raise NotImplementedError("cutout_resize='lanczos3' with several CLIP towers (the resampling tables are built for one tower)")
+    check_tower_options(T, use_augs, cutout_resize)
     if target_embeds is not None:
         if isinstance(target_embeds, th.Tensor):
             if T > 1:

@@ -2,8 +2,9 @@
 
 Replaces the L1 <-> L3 <-> L2 ping-pong the reference executes once per timestep (SURVEY.md 3.2 / 3.3):
 ``p_mean_variance`` + ``cond_fn`` (cgd/cgd.py:151-239) + ``-autograd.grad`` (cgd/cgd.py:228) + the ancestral / DDIM
-update.  One op plan holds both networks and every guidance kernel in a single arena; a whole step is ~1.3k kernel
-launches replayed from one CUDA graph, fed per step by one small pinned H2D copy (scalars, cutout windows, t, y).
+update.  One op plan holds both networks and every guidance kernel in a single arena; a whole step (918 kernel launches for
+bench.py's cfg2: 256², ViT-B/32, 16 cutouts) is replayed from one CUDA graph, fed per step by one small pinned H2D copy (scalars,
+cutout windows, t, y).
 
 Surfaces kept (SURVEY.md 8b): ``cond_fn(x, t, out, y=None)``, ``MakeCutouts``, ``model(x, timesteps, y)``.
 """
@@ -63,7 +64,6 @@ class MakeCutouts(th.nn.Module):
         return self._generate_coords(side_x, side_y, cutn)
 
     def forward(self, input: th.Tensor, use_cache: bool = False, num_cutouts_override: int = None):
-        import ctypes
         if not input.is_cuda:
             raise _lib.CgdError("MakeCutouts.forward runs on the GPU only (no CPU fallback)")
         B, C, H, W = input.shape
@@ -72,36 +72,20 @@ class MakeCutouts(th.nn.Module):
         cs = self.cut_size
         x = input.detach().float().contiguous()
         cdev = th.tensor(coords, dtype=th.int32, device=x.device)
-        lib = _lib.load()
         if self.use_augs:  # the reference applies its augmentations to the raw cutout values: feed 2x - 1, mean 0 / std 1
             from . import augs
             out = th.empty(len(coords) * B, 1, 3 * cs * cs, dtype=th.float16, device=x.device)
             Smax = min(H, W)
             noise = th.zeros(len(coords), 4, B, 3, Smax, Smax, device=x.device)
             prm = augs.draw_aug_params(coords, B, H, W, noise_device=x.device, noise_out=noise).to(x.device)
-            xin = x * 2 - 1
-            op = _lib.CgdOp()
-            op.code = _lib.OP["CUTOUTS_AUG_FWD"]
-            for j, v in enumerate([B, H, W, len(coords), cs, cs, 3 * cs * cs, Smax]):
-                op.i[j] = v
-            for j, v in enumerate([0.0, 0.0, 0.0, 1.0, 1.0, 1.0]):
-                op.f[j] = v
-            for j, t in enumerate([xin, cdev, out, prm, noise]):
-                op.p[j] = t.data_ptr()
-            _lib.check(lib.cgd_run_op(ctypes.byref(op), ctypes.c_void_p(th.cuda.current_stream().cuda_stream)), "cutouts_aug_fwd")
+            _lib.run_op("CUTOUTS_AUG_FWD", i=[B, H, W, len(coords), cs, cs, 3 * cs * cs, Smax], f=[0.0, 0.0, 0.0, 1.0, 1.0, 1.0],
+                        p=[x * 2 - 1, cdev, out, prm, noise])
             return out.view(len(coords) * B, 3, cs, cs).float()
         # mean 0.5 / std 0.5 with the kernel's (x + 1) / 2 yield the raw pooled value; flags 1 = fp32 output like the reference's
         # adaptive_avg_pool2d (the fused step writes fp16 straight into the CLIP tower's patch buffer instead)
         out32 = th.empty(len(coords) * B, 3, cs, cs, dtype=th.float32, device=x.device)
-        op = _lib.CgdOp()
-        op.code, op.flags = _lib.OP["CUTOUTS_FWD"], 1
-        for j, v in enumerate([B, H, W, len(coords), cs, cs, 3 * cs * cs]):
-            op.i[j] = v
-        for j, v in enumerate([0.5, 0.5, 0.5, 0.5, 0.5, 0.5]):
-            op.f[j] = v
-        for j, t in enumerate([x, cdev, out32]):
-            op.p[j] = t.data_ptr()
-        _lib.check(lib.cgd_run_op(ctypes.byref(op), ctypes.c_void_p(th.cuda.current_stream().cuda_stream)), "cgd_cutouts_fwd")
+        _lib.run_op("CUTOUTS_FWD", flags=1, i=[B, H, W, len(coords), cs, cs, 3 * cs * cs], f=[0.5] * 6, p=[x, cdev, out32],
+                    what="cgd_cutouts_fwd")
         return out32
 
 
@@ -154,7 +138,7 @@ class EngineModel:
         for flag in ("grid_gn", "fused_gn", "cluster_splitk"):
             setattr(shadow, flag, getattr(eng.plan, flag))
         UNetB200(eng.unet.cfg, state_dict, batch=eng.B, height=eng.H, width=eng.W, device="cpu", seed_scale=eng.unet.seed_scale, plan=shadow,
-                 build_backward=eng.vit is not None)
+                 build_backward=bool(eng.towers))
         eng.plan.reload_consts(shadow, first=0)  # the UNet is the first network of the engine's plan
         if eng.device.type == "cuda":
             th.cuda.synchronize(eng.device)
@@ -167,16 +151,38 @@ def _as_list(v):
     return list(v) if isinstance(v, (list, tuple)) else [v]
 
 
+def check_tower_options(n_towers: int, use_augs: bool, cutout_resize: str):
+    """several CLIP towers run with the reference's adaptive_avg_pool2d cutouts and no augmentations"""
+    if n_towers > 1 and use_augs:
+        raise NotImplementedError("use_augs with several CLIP towers (the augmentation parameters are drawn for one tower's cutouts)")
+    if n_towers > 1 and cutout_resize == "lanczos3":
+        raise NotImplementedError("cutout_resize='lanczos3' with several CLIP towers (the resampling tables are built for one tower)")
+
+
+def clip_tower(cfg, state_dict, **kw):
+    """the CLIP visual tower of `cfg`: a ViT (vit.py) or a ModifiedResNet (rn.py); both expose patches / embeds / d_embeds / d_patches"""
+    return (RNB200 if isinstance(cfg, RNConfig) else ViTB200)(cfg, state_dict, **kw)
+
+
 class _Tower:
-    """one CLIP tower of the engine: its config, the windows it cuts, its targets, one tower instance per cutout count"""
+    """one CLIP tower of the engine: its config, the buffers of its cutout windows (``coords``) and targets, the slot of its CLIP loss, one tower instance
+    per cutout count, and the ResizeRight tables of its windows"""
 
-    def __init__(self, cfg, coords, targets, vit, tag):
-        self.cfg, self.coords, self.targets, self.vit, self.tag = cfg, coords, targets, vit, tag
-        self.vits = {}
+    def __init__(self, cfg, tag, cutn, coords, targets, loss):
+        self.cfg, self.tag, self.cutn, self.coords, self.targets, self.loss = cfg, tag, cutn, coords, targets, loss
+        self.by_count = {}
+        self.rr = None  # ResizeRight: (left [cutn, cs], weights [cutn, cs, T_MAX], taps [cutn], inverse [cutn, H, 2])
 
-    def sfx(self, count_sfx=""):
+    def sfx(self, c):
         """range-mark suffix: the cutout count's ("@c", "" for the default count), then the tower's ("", "#1", "#2", ...)"""
-        return count_sfx + self.tag
+        return ("" if c == self.cutn else f"@{c}") + self.tag
+
+
+class _Fork(tuple):
+    """schedule entry: the op ranges of one CLIP forward or backward, one per batch slice (vit_streams); run on parallel streams"""
+
+
+ALL_REDUCE = "all_reduce"  # schedule entry: the host all-reduces the partial sums of the sharded RMS clamp (fg_ws) over the ranks
 
 
 class GuidedStepB200:
@@ -204,9 +210,7 @@ class GuidedStepB200:
         sds = _as_list(vit_sd) if vit_cfg is not None else []
         if vit_cfg is not None and (not cfgs or len(sds) != len(cfgs)):
             raise ValueError(f"vit_cfg / vit_sd: one CLIP tower or equal-length non-empty sequences (got {len(cfgs)} configs, {len(sds)} state_dicts)")
-        if len(cfgs) > 1 and (use_augs or cutout_resize != "pool"):
-            raise NotImplementedError("several CLIP towers run with the reference's adaptive_avg_pool2d cutouts and no augmentations "
-                                      "(use_augs and cutout_resize='lanczos3' need per-tower parameters)")
+        check_tower_options(len(cfgs), use_augs, cutout_resize)
         self.T = len(cfgs)
         self.P = max_prompts
         self.scales = dict(cgs=float(clip_guidance_scale), tv=float(tv_scale), rng=float(range_scale), sat=float(sat_scale))
@@ -217,7 +221,7 @@ class GuidedStepB200:
         self.plan = p = Plan(conv_impl=conv_impl)
         B, H, W, HW = self.B, self.H, self.W, self.H * self.W
         self.unet = UNetB200(unet_cfg, unet_sd, batch=B, height=H, width=W, device=device, seed_scale=seed_scale or 1.0, plan=p,
-                             build_backward=vit_cfg is not None)
+                             build_backward=bool(cfgs))
         n3 = B * 3 * HW
         self.sc = p.new(SC["COUNT"], "f", "scalars")
         self.noise = p.new(n3, "f", "noise")
@@ -233,106 +237,61 @@ class GuidedStepB200:
         p.emit("PMV_BLEND", i=[B, HW, 3 * B], p=[(self.unet.x_in, 0), (self.unet.out, 0), (self.sc, 0), (self.x0, 0), (self.mean, 0),
                                                  (self.var, 0), (self.logvar, 0), (self.x_inb, 0), (self.loss, B)], tag="p_mean_variance+blend")
         p.mark("cond")
-        self.vit = None
         self.lpips = None
-        self.use_augs = False
         self.towers = []
         self.loss_towers = None
-        if vit_cfg is not None:
-            vit_cfg, vit_sd = cfgs[0], sds[0]
-            cutn, cs, ps, kp, D = self.cutn, vit_cfg.input_resolution, vit_cfg.patch_size, vit_cfg.kpad, vit_cfg.output_dim
-            self.vit_cfg = vit_cfg
-            self.coords = p.new(cutn * 3, "i32", "cutout_coords")
-            self.targets = p.new(self.P * D, "f", "target_embeds")
-            self.weights = p.new(self.P, "f", "prompt_weights")
-            self.g_clip = p.new(n3, "f", "g_clip")
-            self.dx_direct = p.new(n3, "f", "dx_direct")
-            self.fg_ws = p.new(128, "f", "final_grad_ws")
-            # CLIP visual tower: ViT (vit.py) or ModifiedResNet (rn.py); both expose patches / embeds / d_embeds / d_patches
-            Tower = RNB200 if isinstance(vit_cfg, RNConfig) else ViTB200
-            self.vit = Tower(vit_cfg, vit_sd, n_images=cutn * B, device=device, plan=p, parts=vit_streams)
-            # further cutout counts of the same engine (progressive_cutout, cgd/cgd.py:167-175): own activations and op ranges
-            # ("...@c" marks), shared packed weights; the default count keeps the un-suffixed marks
-            self.vits = {cutn: self.vit}
-            self.towers.append(_Tower(vit_cfg, self.coords, self.targets, self.vit, ""))
-            self.towers[0].vits = self.vits
+        self.use_augs = bool(use_augs and cfgs)
+        # {cutout count: the towers' instances for that count, in tower order}; its keys are the counts the engine runs: num_cutouts and
+        # the further counts of progressive_cutout (cgd/cgd.py:167-175), each with its own activations and op ranges ("...@c" marks),
+        # sharing the packed weights of the default count
+        self.vits = {}
+        if cfgs:
+            cutn = self.cutn
             # cutout resampling: "pool" = adaptive_avg_pool2d like the reference's MakeCutouts (cgd/modules.py:63); "lanczos3" =
             # the vendored ResizeRight resampler north_star names (cgd/ResizeRight/resize_right.py, host tables in resize_right.py)
             if cutout_resize not in ("pool", "lanczos3"):
                 raise ValueError("cutout_resize must be 'pool' or 'lanczos3'")
-            self.cutout_resize = cutout_resize
-            self.use_augs = bool(use_augs)
-            if self.use_augs:
-                if cutout_resize != "pool":
-                    raise NotImplementedError("use_augs runs with the reference's adaptive_avg_pool2d cutouts (cutout_resize='pool')")
+            if use_augs and cutout_resize != "pool":
+                raise NotImplementedError("use_augs runs with the reference's adaptive_avg_pool2d cutouts (cutout_resize='pool')")
+            if cutout_resize == "lanczos3" and (H != W or cutn_variants):
+                raise NotImplementedError("ResizeRight cutouts: square images and a single cutout count only")
+            for c in cutn_variants:
+                if not 0 < int(c) <= cutn:
+                    raise ValueError(f"cutn_variants must lie in (0, {cutn}), got {c}")
+            counts = sorted({cutn, *(int(c) for c in cutn_variants)})
+            self.weights = p.new(self.P, "f", "prompt_weights")
+            self.g_clip = p.new(n3, "f", "g_clip")
+            self.dx_direct = p.new(n3, "f", "dx_direct")
+            self.fg_ws = p.new(128, "f", "final_grad_ws")
+            # clip terms of towers 1..: [T - 1, B] (tower 0's stays in `loss`); SPHERICAL stores them, nothing needs zeroing
+            self.loss_towers = p.new((self.T - 1) * B, "f", "losses_towers") if self.T > 1 else None
+            if use_augs:  # the augmentation parameters of every window and the four noise fields per cutout
                 from .augs import AUG_NP
                 self.aug_smax = min(H, W)
                 self.aug_prm = p.new(cutn * AUG_NP, "f", "aug_params")
                 self.aug_noise = p.new(cutn * 4 * B * 3 * self.aug_smax * self.aug_smax, "f", "aug_noise")
-            if cutout_resize == "lanczos3":
-                if H != W or cutn_variants:
-                    raise NotImplementedError("ResizeRight cutouts: square images and a single cutout count only")
-                from .resize_right import T_MAX
-                # the device tables hold T_MAX = 16 taps per output: lanczos3 with antialiasing needs ceil(6 * S / cs) of them, and the
-                # largest window the reference draws is min(H, W) (cgd/modules.py:40) -- checked here, once, not in the middle of a run
-                if -(-6 * min(H, W) // cs) > T_MAX:
-                    raise ValueError(f"cutout_resize='lanczos3': windows up to {min(H, W)} px down to {cs} px need {-(-6 * min(H, W) // cs)} taps, "
-                                     f"the device tables hold {T_MAX} (images up to {T_MAX * cs // 6} px)")
-                self.rr_left = p.new(cutn * cs, "i32", "rr_left")
-                self.rr_w = p.new(cutn * cs * T_MAX, "f", "rr_weights")
-                self.rr_taps = p.new(cutn, "i32", "rr_taps")
-                self.rr_inv = p.new(cutn * H * 2, "i32", "rr_inverse")
-            variants = sorted(set(int(v) for v in cutn_variants) - {cutn})
-            for c in variants:
-                if not 0 < c < cutn:
-                    raise ValueError(f"cutn_variants must lie in (0, {cutn}), got {c}")
-                self.vits[c] = Tower(vit_cfg, vit_sd, n_images=c * B, device=device, plan=p, parts=vit_streams, suffix=f"@{c}", share=self.vit)
-            # towers 1.. of an ensemble: own windows, targets and activations; range marks suffixed "#m" (tower 0 keeps the plain ones)
-            for m, (cfg_m, sd_m) in enumerate(zip(cfgs[1:], sds[1:]), start=1):
-                Tower_m = RNB200 if isinstance(cfg_m, RNConfig) else ViTB200
-                tw = _Tower(cfg_m, p.new(cutn * 3, "i32", f"cutout_coords#{m}"), p.new(self.P * cfg_m.output_dim, "f", f"target_embeds#{m}"),
-                            None, f"#{m}")
-                tw.vit = Tower_m(cfg_m, sd_m, n_images=cutn * B, device=device, plan=p, parts=vit_streams, suffix=tw.tag)
-                tw.vits[cutn] = tw.vit
-                for c in variants:
-                    tw.vits[c] = Tower_m(cfg_m, sd_m, n_images=c * B, device=device, plan=p, parts=vit_streams, suffix=f"@{c}" + tw.tag, share=tw.vit)
+            for m, (cfg, sd) in enumerate(zip(cfgs, sds)):  # range marks of towers 1.. suffixed "#m", tower 0 keeps the plain ones
+                tag = f"#{m}" if m else ""
+                tw = _Tower(cfg, tag, cutn, p.new(cutn * 3, "i32", "cutout_coords" + tag), p.new(self.P * cfg.output_dim, "f", "target_embeds" + tag),
+                            (self.loss, 0) if m == 0 else (self.loss_towers, (m - 1) * B))
+                cs = cfg.input_resolution
+                if cutout_resize == "lanczos3":
+                    from .resize_right import T_MAX
+                    # the device tables hold T_MAX = 16 taps per output: lanczos3 with antialiasing needs ceil(6 * S / cs) of them, and
+                    # the largest window the reference draws is min(H, W) (cgd/modules.py:40) -- checked here, once, not in the middle of a run
+                    if -(-6 * min(H, W) // cs) > T_MAX:
+                        raise ValueError(f"cutout_resize='lanczos3': windows up to {min(H, W)} px down to {cs} px need {-(-6 * min(H, W) // cs)} "
+                                         f"taps, the device tables hold {T_MAX} (images up to {T_MAX * cs // 6} px)")
+                    tw.rr = (p.new(cutn * cs, "i32", "rr_left"), p.new(cutn * cs * T_MAX, "f", "rr_weights"), p.new(cutn, "i32", "rr_taps"),
+                             p.new(cutn * H * 2, "i32", "rr_inverse"))
+                for c in sorted(counts, key=lambda v: v != cutn):  # the default count first: the others share its weights
+                    tw.by_count[c] = clip_tower(cfg, sd, n_images=c * B, device=device, plan=p, parts=vit_streams, suffix=tw.sfx(c),
+                                                share=tw.by_count.get(cutn))
                 self.towers.append(tw)
-            # clip terms of towers 1..: [T - 1, B] (tower 0's stays in `loss`); SPHERICAL stores them, nothing needs zeroing
-            self.loss_towers = p.new((self.T - 1) * B, "f", "losses_towers") if self.T > 1 else None
+            self.vits = {c: tuple(tw.by_count[c] for tw in self.towers) for c in counts}
             # per cutout count (the default count last: its ranges end at "guide"), then per tower in tower order
-            for c, (m, tw) in itertools.product(sorted(self.vits, key=lambda v: v == cutn), enumerate(self.towers)):
-                sfx, vt = tw.sfx("" if c == cutn else f"@{c}"), tw.vits[c]
-                cs, ps, kp, D = tw.cfg.input_resolution, tw.cfg.patch_size, tw.cfg.kpad, tw.cfg.output_dim
-                coords_m, loss_m = (tw.coords, 0), ((self.loss, 0) if m == 0 else (self.loss_towers, (m - 1) * B))
-                p.mark("cut_fwd" + sfx)
-                if cutout_resize == "lanczos3":
-                    p.emit("CUTOUTS_RR_FWD", i=[B, H, W, c, cs, ps, kp], f=[*CLIP_MEAN, *CLIP_STD],
-                           p=[(self.x_inb, 0), (self.coords, 0), (vt.patches, 0), (self.rr_left, 0), (self.rr_w, 0), (self.rr_taps, 0)],
-                           tag="make_cutouts(resize_right lanczos3)+normalize")
-                elif self.use_augs:
-                    p.emit("CUTOUTS_AUG_FWD", i=[B, H, W, c, cs, ps, kp, self.aug_smax], f=[*CLIP_MEAN, *CLIP_STD],
-                           p=[(self.x_inb, 0), (self.coords, 0), (vt.patches, 0), (self.aug_prm, 0), (self.aug_noise, 0)],
-                           tag="make_cutouts(use_augs)+normalize")
-                else:
-                    p.emit("CUTOUTS_FWD", i=[B, H, W, c, cs, ps, kp], f=[*CLIP_MEAN, *CLIP_STD], p=[(self.x_inb, 0), coords_m, (vt.patches, 0)],
-                           tag="make_cutouts+normalize")
-                p.mark("sph" + sfx)
-                p.emit("SPHERICAL", i=[c, B, self.P, D], f=[self.scales["cgs"], self.vit_grad_scale],
-                       p=[(vt.embeds, 0), (tw.targets, 0), (self.weights, 0), (vt.d_embeds, 0), loss_m], tag="spherical_dist_loss")
-                p.mark("cut_bwd" + sfx)
-                if cutout_resize == "lanczos3":
-                    p.emit("CUTOUTS_RR_BWD", i=[B, H, W, c, cs, ps, kp, H], f=[0, 0, 0, *CLIP_STD, 1.0 / self.vit_grad_scale],
-                           p=[(vt.d_patches, 0), (self.coords, 0), (self.g_clip, 0), (self.rr_left, 0), (self.rr_w, 0), (self.rr_inv, 0)],
-                           tag="d_make_cutouts(resize_right)")
-                elif self.use_augs:
-                    p.emit("FILL", i=[n3], f=[0.0], p=[(self.g_clip, 0)], tag="zero g_clip")
-                    p.emit("CUTOUTS_AUG_BWD", i=[B, H, W, c, cs, ps, kp], f=[0, 0, 0, *CLIP_STD, 1.0 / self.vit_grad_scale],
-                           p=[(vt.d_patches, 0), (self.coords, 0), (self.g_clip, 0), (self.aug_prm, 0)], tag="d_make_cutouts(use_augs)")
-                else:
-                    # tower 0 stores the x_in gradient, towers 1.. add theirs (flags 2) in tower order: a deterministic sum
-                    p.emit("CUTOUTS_BWD", flags=0 if m == 0 else 2, i=[B, H, W, c, cs, ps, kp], f=[0, 0, 0, *CLIP_STD, 1.0 / self.vit_grad_scale],
-                           p=[(vt.d_patches, 0), coords_m, (self.g_clip, 0)], tag="d_make_cutouts")
-                p.mark("cut_end" + sfx)
+            for c, (m, tw) in itertools.product(sorted(counts, key=lambda v: v == cutn), enumerate(self.towers)):
+                self._emit_cutouts(tw, c, accumulate=m > 0)
             if lpips_sd is not None and init_scale != 0:
                 from .lpips import LpipsB200
                 # d (init_scale * lpips_vgg(x_in, init).sum()) / d x_in is added to the x_in gradient the cutout backward left in g_clip
@@ -373,23 +332,58 @@ class GuidedStepB200:
         p.finalize(device)
         self.model = EngineModel(self)
         self.shape = (B, 3, H, W)
-        # pinned staging for the per-step host->device refresh
-        self._n_stage = SC["COUNT"] * 4 + self.cutn * 3 * 4 + B * 4 + B * 8 + self.cutn * 20 * 4 + max(self.T - 1, 0) * self.cutn * 3 * 4
-        # The host runs ahead of the GPU (a step is ~1 ms of host work and ~10 ms of device work, and nothing synchronises between
-        # saved frames), so the async copies of step k may still be queued when the host stages step k+1: the pinned buffers are a
-        # ring of STAGE_SLOTS slots, each guarded by the event recorded after its copies were enqueued.
+        # The pinned staging slot of a step: one region per device buffer the host uploads, in this order (int64 classes first, for
+        # alignment).  The host runs ahead of the GPU (a step is ~1 ms of host work and ~10 ms of device work, and nothing
+        # synchronises between saved frames), so the async copies of step k may still be queued when the host stages step k+1: the
+        # slots are a ring of STAGE_SLOTS, each guarded by the event recorded after its copies were enqueued.
+        staged = [self.unet.y_in, self.sc, self.unet.t_in] + ([self.aug_prm] if self.use_augs else [])
+        for tw in self.towers:
+            staged += [tw.coords] + list(tw.rr or ())
+        self._slot, size = {}, 0
+        for b in staged:  # arena offset of the device buffer -> offset of its region in the slot
+            self._slot[b.off], size = size, size + b.nbytes
         pin = self.device.type == "cuda"
-        self._stage_ring = [th.zeros(self._n_stage, dtype=th.uint8, pin_memory=pin) for _ in range(self.STAGE_SLOTS)]
+        self._stage_ring = [th.zeros(size, dtype=th.uint8, pin_memory=pin) for _ in range(self.STAGE_SLOTS)]
         self._stage_events = [None] * self.STAGE_SLOTS
         self._stage_i = 0
-        self._rr_ring = None
         self._graphs = {}
-        self._side_streams = [th.cuda.Stream(device=self.device) for _ in range(max((tw.vit.parts for tw in self.towers), default=1) - 1)] \
-            if self.device.type == "cuda" else []
+        self._side_streams = [th.cuda.Stream(device=self.device) for _ in range(max((vt.parts for vt in self.vits.get(self.cutn, ())),
+                                                                                    default=1) - 1)] if self.device.type == "cuda" else []
         self._last_out = None
         self._fwd_valid = False
         self.h2d_bytes = 0
         self.d2h_bytes = 0
+
+    def _emit_cutouts(self, tw, c, accumulate):
+        """cutouts -> CLIP (the tower's own op ranges) -> spherical loss -> cutout gradient into g_clip, for `c` windows of tower `tw`;
+        `accumulate`: add to g_clip (towers 1..) instead of storing (tower 0), a deterministic sum in tower order"""
+        p, B, H, W = self.plan, self.B, self.H, self.W
+        sfx, vt = tw.sfx(c), tw.by_count[c]
+        cs, ps, kp, D = tw.cfg.input_resolution, tw.cfg.patch_size, tw.cfg.kpad, tw.cfg.output_dim
+        dims, win = [B, H, W, c, cs, ps, kp], (tw.coords, 0)
+        fwd_f, bwd_f = [*CLIP_MEAN, *CLIP_STD], [0, 0, 0, *CLIP_STD, 1.0 / self.vit_grad_scale]
+        p.mark("cut_fwd" + sfx)
+        if tw.rr:
+            p.emit("CUTOUTS_RR_FWD", i=dims, f=fwd_f, p=[(self.x_inb, 0), win, (vt.patches, 0), *((b, 0) for b in tw.rr[:3])],
+                   tag="make_cutouts(resize_right lanczos3)+normalize")
+        elif self.use_augs:
+            p.emit("CUTOUTS_AUG_FWD", i=dims + [self.aug_smax], f=fwd_f, p=[(self.x_inb, 0), win, (vt.patches, 0), (self.aug_prm, 0), (self.aug_noise, 0)],
+                   tag="make_cutouts(use_augs)+normalize")
+        else:
+            p.emit("CUTOUTS_FWD", i=dims, f=fwd_f, p=[(self.x_inb, 0), win, (vt.patches, 0)], tag="make_cutouts+normalize")
+        p.mark("sph" + sfx)
+        p.emit("SPHERICAL", i=[c, B, self.P, D], f=[self.scales["cgs"], self.vit_grad_scale],
+               p=[(vt.embeds, 0), (tw.targets, 0), (self.weights, 0), (vt.d_embeds, 0), tw.loss], tag="spherical_dist_loss")
+        p.mark("cut_bwd" + sfx)
+        if tw.rr:
+            p.emit("CUTOUTS_RR_BWD", i=dims + [H], f=bwd_f, p=[(vt.d_patches, 0), win, (self.g_clip, 0), (tw.rr[0], 0), (tw.rr[1], 0), (tw.rr[3], 0)],
+                   tag="d_make_cutouts(resize_right)")
+        elif self.use_augs:
+            p.emit("FILL", i=[B * 3 * H * W], f=[0.0], p=[(self.g_clip, 0)], tag="zero g_clip")
+            p.emit("CUTOUTS_AUG_BWD", i=dims, f=bwd_f, p=[(vt.d_patches, 0), win, (self.g_clip, 0), (self.aug_prm, 0)], tag="d_make_cutouts(use_augs)")
+        else:
+            p.emit("CUTOUTS_BWD", flags=2 if accumulate else 0, i=dims, f=bwd_f, p=[(vt.d_patches, 0), win, (self.g_clip, 0)], tag="d_make_cutouts")
+        p.mark("cut_end" + sfx)
 
     # ------------------------------------------------------------------ views
     def v(self, buf, shape=None):
@@ -458,6 +452,58 @@ class GuidedStepB200:
         full = th.randint(0, self.unet.num_classes, (self.global_batch,), device=self.device)
         return self.local_rows(full)
 
+    # ------------------------------------------------------------------ the step's op ranges
+    def schedule(self, mode, cutn=None, guided=True) -> list:
+        """The op ranges of one step in launch order: (mark_a, mark_b) pairs, a ``_Fork`` for the CLIP forward and the CLIP backward of
+        each tower, and ``ALL_REDUCE`` where the sharded RMS clamp all-reduces its partial sums.  A guided step runs UNet forward ->
+        p_mean_variance -> per tower (cutouts, CLIP fwd, loss, CLIP bwd, cutout gradient) -> LPIPS -> tv / range / sat -> UNet dgrad ->
+        -grad (+ clamp) -> update; an unguided one (reduce_clip's skipped steps) UNet forward -> p_mean_variance -> update."""
+        steps = [("unet_emb", "unet_bwd"), ("pmv", "cond")]
+        if guided and self.towers:
+            c = self.cutn if cutn is None else cutn
+            if c not in self.vits:
+                raise ValueError(f"engine built for cutout counts {sorted(self.vits)}, got {cutn}")
+            for tw in self.towers:
+                sfx, vt = tw.sfx(c), tw.by_count[c]
+                steps += [("cut_fwd" + sfx, "sph" + sfx), _Fork(vt.part_ranges("fwd")), ("sph" + sfx, "cut_bwd" + sfx),
+                          _Fork(vt.part_ranges("bwd")), ("cut_bwd" + sfx, "cut_end" + sfx)]
+            steps += [("lpips", "lpips_end")] if self.lpips is not None else []
+            steps += [("guide", "final"), ("unet_bwd", "unet_end")]
+            steps += [("final", "mag"), ALL_REDUCE, ("mag", "upd_anc_g")] if self.mag_sync else [("final", "upd_anc_g")]
+        if mode == "ancestral":
+            return steps + [("upd_anc_g", "upd_anc") if guided else ("upd_anc", "upd_ddim_g")]
+        return steps + [("upd_ddim_g", "upd_ddim") if guided else ("upd_ddim", "engine_end")]
+
+    def _run_all(self, mode, runner=None, cutn=None):
+        """one guided step launched range by range, without a CUDA graph; ``runner(mark_a, mark_b)`` stands in for
+        ``plan.run_range`` (the tests interpret op lists with it)"""
+        self._launch(self.schedule(mode, cutn), runner)
+
+    def _launch(self, steps, runner=None):
+        run = runner or self.plan.run_range
+        for e in steps:
+            if e == ALL_REDUCE:
+                import torch.distributed as dist
+                dist.all_reduce(self.v(self.fg_ws))
+            elif isinstance(e, _Fork) and len(e) > 1 and runner is None and self._side_streams:
+                # one CLIP pass per batch slice on parallel streams (fork / join around the current stream; inside CUDA-graph capture
+                # this becomes parallel branches of the graph)
+                main = th.cuda.current_stream()
+                for s, (a, b) in zip(self._side_streams, e[1:]):
+                    s.wait_stream(main)
+                    self.plan.run_range(a, b, stream=s.cuda_stream)
+                self.plan.run_range(*e[0])
+                for s in self._side_streams:
+                    main.wait_stream(s)
+            else:
+                for a, b in (e if isinstance(e, _Fork) else [e]):
+                    run(a, b)
+
+    def launches_per_step(self, mode="ddim") -> int:
+        m = self.plan.marks
+        ranges = [r for e in self.schedule(mode) if e != ALL_REDUCE for r in (e if isinstance(e, _Fork) else [e])]
+        return sum(self.plan.num_launches(m[a], m[b] - m[a]) for a, b in ranges)
+
     # ------------------------------------------------------------------ segment-wise execution (API-parity path)
     def _push_scalars(self, sc: np.ndarray):
         self.v(self.sc).copy_(th.from_numpy(sc), non_blocking=True)
@@ -469,8 +515,7 @@ class GuidedStepB200:
         self._push_scalars(diffusion.scalar_table(t_index, fac_index))
         ts = th.full((self.B,), diffusion.model_timestep(t_index), dtype=th.float32)
         self.unet.set_inputs(x, ts.to(self.device, non_blocking=True), y)
-        self.plan.run_range("unet_emb", "unet_bwd")
-        self.plan.run_range("pmv", "cond")
+        self._launch(self.schedule("ddim", guided=False)[:2])  # UNet forward, p_mean_variance
         self._fwd_valid = True
         out = {"mean": self.img(self.mean), "variance": self.img(self.var), "log_variance": self.img(self.logvar),
                "pred_xstart": self.img(self.x0), "engine": self}
@@ -481,41 +526,18 @@ class GuidedStepB200:
         """-d(loss)/dx for the last unet_forward (what cond_fn returns)."""
         if not self._fwd_valid:
             raise RuntimeError("cond_fn called without a preceding p_mean_variance on this engine")
-        if self.vit is None:
+        if not self.towers:
             raise RuntimeError("engine built without a CLIP tower")
         if fac_index != self._cur_t:  # quirk B2: fac follows the closure's current_timestep, not t
             sc = diffusion.scalar_table(self._cur_t, fac_index)
             self._push_scalars(sc)
             self.plan.run_range("pmv", "cond")
-        per = self._per_tower(coords)
-        cutn = len(per[0])
-        csfx = self._sfx(cutn)
-        for tw, cm in zip(self.towers, per):
-            self.v(tw.coords, (self.cutn, 3))[:cutn].copy_(th.tensor(cm, dtype=th.int32), non_blocking=True)
-        self._stage_resize_tables(per[0])
-        if self.use_augs:
-            self._stage_augs(per[0])
-        for m, tw in enumerate(self.towers):
-            sfx = tw.sfx(csfx)
-            self.plan.run_range("cut_fwd" + sfx, "sph" + sfx)
-            self._run_vit("fwd", None, cutn, m)
-            self.plan.run_range("sph" + sfx, "cut_bwd" + sfx)
-            self._run_vit("bwd", None, cutn, m)
-            self.plan.run_range("cut_bwd" + sfx, "cut_end" + sfx)
-        for a, b in ((("lpips", "lpips_end"),) if self.lpips is not None else ()) + (("guide", "final"), ("unet_bwd", "unet_end")):
-            self.plan.run_range(a, b)
-        self._run_final(self.plan.run_range)
+        steps = self.schedule("ddim", len(self._per_tower(coords)[0]))[2:-1]  # the guidance between p_mean_variance and the update
+        k = self._stage_acquire()
+        self._stage_windows(self._stage_ring[k], coords)
+        self._stage_release(k)
+        self._launch(steps)
         return self.img(self.g)
-
-    def _run_final(self, pr):
-        """-grad (+ RMS clamp).  Sharded batch with use_magnitude: partial sums -> all-reduce over ranks -> clamp."""
-        if not self.mag_sync:
-            pr("final", "upd_anc_g")
-            return
-        import torch.distributed as dist
-        pr("final", "mag")
-        dist.all_reduce(self.v(self.fg_ws))
-        pr("mag", "upd_anc_g")
 
     def update(self, diffusion, mode, t_index, g, noise, eta=0.0) -> th.Tensor:
         if mode == "ddim" and eta != 0.0:
@@ -524,23 +546,14 @@ class GuidedStepB200:
             self.img(self.noise).copy_(noise)
         if g is not None and g.data_ptr() != self.v(self.g).data_ptr():
             self.img(self.g).copy_(g)
-        name = ("upd_anc" if mode == "ancestral" else "upd_ddim") + ("_g" if g is not None else "")
-        order = ["upd_anc_g", "upd_anc", "upd_ddim_g", "upd_ddim", "engine_end"]
-        self.plan.run_range(name, order[order.index(name) + 1])
+        self._launch(self.schedule(mode, guided=g is not None)[-1:])
         self._fwd_valid = False
         return self.img(self.sample).clone()
 
-    # ------------------------------------------------------------------ fused step (one CUDA graph)
+    # ------------------------------------------------------------------ fused step (CUDA graphs)
     def can_fuse(self, cond_fn, clip_denoised, denoised_fn) -> bool:
         return (isinstance(cond_fn, CondFnB200) and cond_fn.engine is self and not clip_denoised and denoised_fn is None
                 and cond_fn.fusable())
-
-    def _sfx(self, cutn):
-        if cutn is None or cutn == self.cutn:
-            return ""
-        if cutn not in self.vits:
-            raise ValueError(f"engine built for cutout counts {sorted(self.vits)}, got {cutn}")
-        return f"@{cutn}"
 
     def _per_tower(self, coords):
         """a step's cutout windows -> one window list per tower: one tower takes a flat window list, an ensemble a sequence of
@@ -552,61 +565,6 @@ class GuidedStepB200:
             raise ValueError(f"engine built with {self.T} CLIP towers: expected {self.T} window lists of one length, got "
                              f"{[len(c) for c in per]}")
         return per
-
-    def _run_all(self, mode, runner=None, cutn=None, part=None):
-        pr = runner or self.plan.run_range
-        csfx = self._sfx(cutn)
-        pr("unet_emb", "unet_bwd")
-        pr("pmv", "cond")
-        for m, tw in enumerate(self.towers):  # one tower after another: cutouts -> fwd -> loss -> bwd -> cutout gradient
-            sfx = tw.sfx(csfx)
-            pr("cut_fwd" + sfx, "sph" + sfx)
-            self._run_vit("fwd", pr, cutn, m)
-            pr("sph" + sfx, "cut_bwd" + sfx)
-            self._run_vit("bwd", pr, cutn, m)
-            pr("cut_bwd" + sfx, "cut_end" + sfx)
-        if self.lpips is not None:
-            pr("lpips", "lpips_end")
-        pr("guide", "final")
-        pr("unet_bwd", "unet_end")
-        if part == "A":  # everything up to the partial sums of the sharded RMS clamp (see replay)
-            pr("final", "mag")
-            return
-        self._run_final(pr)
-        self._run_update(mode, pr)
-
-    def _run_update(self, mode, pr):
-        if mode == "ancestral":
-            pr("upd_anc_g", "upd_anc")
-        else:
-            pr("upd_ddim_g", "upd_ddim")
-
-    def _run_vit(self, which, pr=None, cutn=None, tower=0):
-        """CLIP forward / backward of one tower: one op range, or one per batch slice on parallel streams (fork / join around the
-        current stream; inside CUDA-graph capture this becomes parallel branches of the graph)."""
-        pr = pr or self.plan.run_range
-        ranges = self.towers[tower].vits[self.cutn if cutn is None else cutn].part_ranges(which)
-        if len(ranges) == 1 or not self._side_streams or pr != self.plan.run_range:
-            for a, b in ranges:
-                pr(a, b)
-            return
-        main = th.cuda.current_stream()
-        for s, (a, b) in zip(self._side_streams, ranges[1:]):
-            s.wait_stream(main)
-            self.plan.run_range(a, b, stream=s.cuda_stream)
-        self.plan.run_range(*ranges[0])
-        for s in self._side_streams:
-            main.wait_stream(s)
-
-    def launches_per_step(self, mode="ddim") -> int:
-        m = self.plan.marks
-        segs = [("unet_emb", "unet_bwd"), ("pmv", "cond")] + [
-                (a + t, b + t) for t in (tw.tag for tw in self.towers) for a, b in (
-                    ("cut_fwd", "sph"), ("vit_fwd", "vit_bwd"), ("sph", "cut_bwd"), ("vit_bwd", "vit_end"), ("cut_bwd", "cut_end"))] + (
-                [("lpips", "lpips_end")] if self.lpips is not None else []) + [
-                ("guide", "final"), ("unet_bwd", "unet_end"), ("final", "upd_anc_g"),
-                ("upd_anc_g", "upd_anc") if mode == "ancestral" else ("upd_ddim_g", "upd_ddim")]  # "mag" lies inside (final, upd_anc_g)
-        return sum(self.plan.num_launches(m[a], m[b] - m[a]) for a, b in segs)
 
     STAGE_SLOTS = 4
 
@@ -625,96 +583,82 @@ class GuidedStepB200:
             ev.record(th.cuda.current_stream(self.device))
             self._stage_events[k] = ev
 
+    def _region(self, st, buf, dtype):
+        """the region of device buffer `buf` in the pinned slot `st`, as `dtype`"""
+        o = self._slot[buf.off]
+        return st[o:o + buf.nbytes].view(dtype)
+
+    def _upload(self, st, buf, nbytes=None):
+        """async copy of the first `nbytes` (all) of buf's region of the slot `st` into the device buffer"""
+        o, n = self._slot[buf.off], buf.nbytes if nbytes is None else nbytes
+        self.plan.arena[buf.off:buf.off + n].copy_(st[o:o + n], non_blocking=True)
+        self.h2d_bytes += n
+
     def stage_step(self, sc: np.ndarray, coords, t_model: float, y=None):
         """One pinned staging slot -> small async H2D copies (classes, scalars, timestep, cutout windows)."""
         k = self._stage_acquire()
         st = self._stage_ring[k]
-        o = self.B * 8  # [0, 8B): int64 classes (kept first for alignment)
         self.h2d_bytes = 0
         if y is not None and self.unet.cfg.class_cond:
             if y.device.type == "cpu":
-                st[0:o].view(th.int64).copy_(y)
-                self.v(self.unet.y_in).view(th.uint8).copy_(st[0:o], non_blocking=True)
-                self.h2d_bytes += o
+                self._region(st, self.unet.y_in, th.int64).copy_(y)
+                self._upload(st, self.unet.y_in)
             else:
                 self.v(self.unet.y_in).copy_(y)
-        n = SC["COUNT"] * 4
-        st[o:o + n].view(th.float32).copy_(th.from_numpy(sc))
-        self.v(self.sc).view(th.uint8).copy_(st[o:o + n], non_blocking=True)
-        o += n
-        n = self.B * 4
-        st[o:o + n].view(th.float32).fill_(t_model)
-        self.v(self.unet.t_in).view(th.uint8).copy_(st[o:o + n], non_blocking=True)
-        o += n
-        self.h2d_bytes += SC["COUNT"] * 4 + self.B * 4
-        per = self._per_tower(coords) if self.cutn else []
-        if self.cutn:
-            for ox, oy, size in itertools.chain(*per):  # windows may be clipped at the border (quirk B3) but not empty
-                if not (0 <= ox < self.W and 0 <= oy < self.H and size > 0):
-                    raise RuntimeError(f"cutout window (x={ox}, y={oy}, size={size}) lies outside the {self.H}x{self.W} image: the reference's "
-                                       "adaptive_avg_pool2d raises on the empty crop (non-square images, cgd/modules.py:52,61)")
-            n = len(per[0]) * 12
-        if self.cutn and len(per[0]):
-            coords = per[0]
-            st[o:o + n].view(th.int32).copy_(th.tensor(coords, dtype=th.int32).view(-1))
-            self.v(self.coords).view(th.uint8)[:n].copy_(st[o:o + n], non_blocking=True)
-            self.h2d_bytes += n
-            o += self.cutn * 12
-            self._stage_resize_tables(coords, k)
-            if getattr(self, "use_augs", False):
-                self._stage_augs(coords, st, o)
-            o += self.cutn * 20 * 4
-            for tw, cm in zip(self.towers[1:], per[1:]):  # the other towers' windows follow the use_augs region
-                st[o:o + n].view(th.int32).copy_(th.tensor(cm, dtype=th.int32).view(-1))
-                self.v(tw.coords).view(th.uint8)[:n].copy_(st[o:o + n], non_blocking=True)
-                self.h2d_bytes += n
-                o += self.cutn * 12
+        self._region(st, self.sc, th.float32).copy_(th.from_numpy(sc))
+        self._upload(st, self.sc)
+        self._region(st, self.unet.t_in, th.float32).fill_(t_model)
+        self._upload(st, self.unet.t_in)
+        self._stage_windows(st, coords)
         self._stage_release(k)
 
-    def _stage_augs(self, coords, st=None, o=0):
+    def _stage_windows(self, st, coords):
+        """every tower's cutout windows of this step (and the use_augs parameters / ResizeRight tables drawn or built from them) ->
+        the pinned slot `st` -> the device; an unguided step has none"""
+        if not self.towers:
+            return
+        per = self._per_tower(coords)
+        for ox, oy, size in itertools.chain(*per):  # windows may be clipped at the border (quirk B3) but not empty
+            if not (0 <= ox < self.W and 0 <= oy < self.H and size > 0):
+                raise RuntimeError(f"cutout window (x={ox}, y={oy}, size={size}) lies outside the {self.H}x{self.W} image: the reference's "
+                                   "adaptive_avg_pool2d raises on the empty crop (non-square images, cgd/modules.py:52,61)")
+        for tw, windows in zip(self.towers, per):
+            if not windows:
+                continue
+            w = th.tensor(windows, dtype=th.int32).view(-1)
+            self._region(st, tw.coords, th.int32)[:w.numel()].copy_(w)
+            self._upload(st, tw.coords, w.numel() * 4)
+            if self.use_augs:
+                self._stage_augs(st, windows)
+            if tw.rr:
+                self._stage_resize_tables(st, tw, windows)
+
+    def _stage_augs(self, st, windows):
         """use_augs: this step's flip / affine / perspective / grayscale parameters (CPU generator, torchvision's order) and the four
         noise fields per cutout (device generator, the reference's shapes; full batch drawn, own rows kept when sharded)"""
         from . import augs
-        n = len(coords) * augs.AUG_NP * 4
-        noise = self.v(self.aug_noise, (self.cutn, 4, self.B, 3, self.aug_smax, self.aug_smax))
+        S = self.aug_smax
+        noise = self.v(self.aug_noise, (self.cutn, 4, self.B, 3, S, S))
         rows = None if self.world == 1 else (self.rank * self.B, (self.rank + 1) * self.B)
-        prm = augs.draw_aug_params(coords, self.global_batch, self.H, self.W, noise_device=self.device, noise_out=noise, rows=rows)
-        dst = self.v(self.aug_prm).view(th.uint8)[:n]
-        if st is None:
-            dst.copy_(prm.view(-1).view(th.uint8))
-        else:
-            st[o:o + n].view(th.float32).copy_(prm.view(-1))
-            dst.copy_(st[o:o + n], non_blocking=True)
-        self.h2d_bytes += n
+        prm = augs.draw_aug_params(windows, self.global_batch, self.H, self.W, noise_device=self.device, noise_out=noise, rows=rows).view(-1)
+        self._region(st, self.aug_prm, th.float32)[:prm.numel()].copy_(prm)
+        self._upload(st, self.aug_prm, prm.numel() * 4)
 
-    def _stage_resize_tables(self, coords, slot=None):
+    def _stage_resize_tables(self, st, tw, windows):
         """ResizeRight mode: per-cutout resampling tables of this step's crop sizes (cached per size on the host) -> device"""
-        if self.vit is None or self.cutout_resize != "lanczos3":
-            return
         from . import resize_right as rr
-        cs, S_max = self.vit_cfg.input_resolution, self.H
-        if self._rr_ring is None:
-            pin = self.device.type == "cuda"
-            self._rr_ring = [(th.zeros(self.cutn, cs, dtype=th.int32, pin_memory=pin), th.zeros(self.cutn, cs, rr.T_MAX, pin_memory=pin),
-                              th.zeros(self.cutn, dtype=th.int32, pin_memory=pin), th.zeros(self.cutn, S_max, 2, dtype=th.int32, pin_memory=pin))
-                             for _ in range(self.STAGE_SLOTS)]
-        own = slot is None  # segment path (cond_grad): take and guard a slot of its own
-        if own:
-            slot = self._stage_acquire()
-        pl, pw, pt, pi_ = self._rr_ring[slot]
-        for k, (_, _, S) in enumerate(coords):
-            left, w, T = rr.tables(int(S), cs)
-            pl[k].copy_(left)
+        cs, n = tw.cfg.input_resolution, self.cutn
+        left, wts, taps, inv = tw.rr
+        pl, pw = self._region(st, left, th.int32).view(n, cs), self._region(st, wts, th.float32).view(n, cs, rr.T_MAX)
+        pt, pi_ = self._region(st, taps, th.int32), self._region(st, inv, th.int32).view(n, self.H, 2)
+        for k, (_, _, S) in enumerate(windows):
+            l, w, T = rr.tables(int(S), cs)
+            pl[k].copy_(l)
             pw[k].copy_(w)
             pt[k] = T
-            pi_[k, :S].copy_(rr.inverse_ranges(left, T, int(S)))
-        self.v(self.rr_left, (self.cutn, cs)).copy_(pl, non_blocking=True)
-        self.v(self.rr_w, (self.cutn, cs, rr.T_MAX)).copy_(pw, non_blocking=True)
-        self.v(self.rr_taps, (self.cutn,)).copy_(pt, non_blocking=True)
-        self.v(self.rr_inv, (self.cutn, S_max, 2)).copy_(pi_, non_blocking=True)
-        self.h2d_bytes += pl.numel() * 4 + pw.numel() * 4 + pt.numel() * 4 + pi_.numel() * 4
-        if own:
-            self._stage_release(slot)
+            pi_[k, :S].copy_(rr.inverse_ranges(l, T, int(S)))
+        for b in tw.rr:
+            self._upload(st, b)
 
     def fused_step(self, diffusion, mode, t_index, img, y, cond_fn, eta=0.0) -> dict:
         # RNG order of the reference: the ancestral sampler draws its noise BEFORE cond_fn (whose MakeCutouts draws the windows
@@ -738,62 +682,28 @@ class GuidedStepB200:
         self.replay(mode, len(self._per_tower(coords)[0]) if (self.cutn and guided) else None, guided=guided)
         return {"sample": self.img(self.sample).clone(), "pred_xstart": self.img(self.x0).clone()}
 
-    def _run_unguided(self, mode, pr=None):
-        """a step whose guidance gradient is zero (reduce_clip's skipped steps): UNet forward, p_mean_variance, plain update"""
-        pr = pr or self.plan.run_range
-        pr("unet_emb", "unet_bwd")
-        pr("pmv", "cond")
-        if mode == "ancestral":
-            pr("upd_anc", "upd_ddim_g")
-        else:
-            pr("upd_ddim", "engine_end")
-
     def replay(self, mode, cutn=None, guided=True):
-        if cutn == self.cutn:
-            cutn = None
-        if not guided:
-            if not self.use_graph:
-                self._run_unguided(mode)
-                return
-            g = self._graphs.get((mode, "unguided"))
-            if g is None:
-                self._run_unguided(mode)
-                th.cuda.synchronize()
-                g = th.cuda.CUDAGraph()
-                with th.cuda.graph(g):
-                    self._run_unguided(mode)
-                self._graphs[(mode, "unguided")] = g
-            g.replay()
-            return
+        """one step from CUDA graphs: the schedule cut at its host all-reduce into segments, one graph per segment, captured on first
+        use after one eager run (which sets kernel attributes and touches every buffer), then replayed with the all-reduce between"""
+        steps = self.schedule(mode, cutn, guided)
         if not self.use_graph:
-            self._run_all(mode, None, cutn)
+            self._launch(steps)
             return
-        if self.mag_sync:  # two graphs around the all-reduce of the RMS partial sums
-            import torch.distributed as dist
-            gs = self._graphs.get((mode, cutn))
-            if gs is None:
-                self._run_all(mode, None, cutn)
-                th.cuda.synchronize()
-                ga, gb = th.cuda.CUDAGraph(), th.cuda.CUDAGraph()
-                with th.cuda.graph(ga):
-                    self._run_all(mode, None, cutn, part="A")
-                with th.cuda.graph(gb):
-                    self.plan.run_range("mag", "upd_anc_g")
-                    self._run_update(mode, self.plan.run_range)
-                gs = self._graphs[(mode, cutn)] = (ga, gb)
-            gs[0].replay()
-            dist.all_reduce(self.v(self.fg_ws))
-            gs[1].replay()
-            return
-        g = self._graphs.get((mode, cutn))
-        if g is None:
-            self._run_all(mode, None, cutn)  # warm-up: sets kernel attributes, touches every buffer
+        key = (mode, (None if cutn == self.cutn else cutn) if guided else "unguided")
+        graphs = self._graphs.get(key)
+        if graphs is None:
+            self._launch(steps)
             th.cuda.synchronize()
-            g = th.cuda.CUDAGraph()
-            with th.cuda.graph(g):
-                self._run_all(mode, None, cutn)
-            self._graphs[(mode, cutn)] = g
-        g.replay()
+            graphs = self._graphs[key] = []
+            cuts = [-1] + [k for k, e in enumerate(steps) if e == ALL_REDUCE] + [len(steps)]
+            for a, b in zip(cuts, cuts[1:]):
+                graphs.append(th.cuda.CUDAGraph())
+                with th.cuda.graph(graphs[-1]):
+                    self._launch(steps[a + 1:b])
+        for k, g in enumerate(graphs):
+            if k:
+                self._launch([ALL_REDUCE])
+            g.replay()
 
     def losses(self) -> dict:
         """per-image loss terms of the last step (device->host sync; logging only, like tqdm.write at cgd/cgd.py:234-236)"""

@@ -16,15 +16,11 @@ is unambiguous and runs here, once per image prompt and run, outside the samplin
 """
 from __future__ import annotations
 
-import ctypes
-
 import numpy as np
 import torch as th
 
 from . import _lib
-from .guidance import CLIP_MEAN, CLIP_STD, MakeCutouts
-from .rn import RNB200, RNConfig
-from .vit import ViTB200
+from .guidance import CLIP_MEAN, CLIP_STD, MakeCutouts, clip_tower
 
 
 def check_local(path: str):
@@ -52,15 +48,7 @@ def resized_shape(height: int, width: int, diffusion_size: int) -> "tuple[int, i
 
 
 def _run_op(code: str, i, f=(), p=()):
-    op = _lib.CgdOp()
-    op.code = _lib.OP[code]
-    for j, v in enumerate(i):
-        op.i[j] = int(v)
-    for j, v in enumerate(f):
-        op.f[j] = float(v)
-    for j, t in enumerate(p):
-        op.p[j] = t.data_ptr()
-    _lib.check(_lib.load().cgd_run_op(ctypes.byref(op), ctypes.c_void_p(th.cuda.current_stream().cuda_stream)), code.lower())
+    _lib.run_op(code, i=i, f=f, p=p)
 
 
 def resize_lanczos3(x: th.Tensor, out_hw: "tuple[int, int]") -> th.Tensor:
@@ -92,8 +80,7 @@ class ImagePromptEncoder:
 
     def __init__(self, tower_cfg, clip_sd: dict, num_cutouts: int, device="cuda"):
         self.cfg, self.cutn, self.device = tower_cfg, int(num_cutouts), th.device(device)
-        Tower = RNB200 if isinstance(tower_cfg, RNConfig) else ViTB200
-        self.tower = Tower(tower_cfg, clip_sd, n_images=self.cutn, device=device, build_backward=False)
+        self.tower = clip_tower(tower_cfg, clip_sd, n_images=self.cutn, device=device, build_backward=False)
         self.make_cutouts = MakeCutouts(cut_size=tower_cfg.input_resolution, num_cutouts=self.cutn)
         self.last = {}  # resized image and cutout windows of the last call (inspection / tests)
 

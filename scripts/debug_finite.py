@@ -11,6 +11,7 @@ th.manual_seed(0)
 img = eng.draw_initial_noise()
 i = diff.num_timesteps - 1
 p = eng.plan
+vt = eng.towers[0].by_count[eng.cutn]  # the (only) CLIP tower at the default cutout count
 
 
 def stat(name, t):
@@ -36,13 +37,13 @@ for step in range(6):
         elif a == "pmv":
             stat("pred_xstart", eng.img(eng.x0)); stat("x_in", eng.img(eng.x_inb))
         elif a == "cut_fwd":
-            stat("patches", p.view(eng.vit.patches))
+            stat("patches", p.view(vt.patches))
         elif a == "vit_fwd":
-            stat("embeds", p.view(eng.vit.embeds))
+            stat("embeds", p.view(vt.embeds))
         elif a == "sph":
-            stat("d_embeds", p.view(eng.vit.d_embeds))
+            stat("d_embeds", p.view(vt.d_embeds))
         elif a == "vit_bwd":
-            stat("d_patches", p.view(eng.vit.d_patches))
+            stat("d_patches", p.view(vt.d_patches))
         elif a == "cut_bwd":
             stat("g_clip", eng.img(eng.g_clip))
         elif a == "guide":

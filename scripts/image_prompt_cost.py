@@ -100,7 +100,7 @@ def time_step(P, steps=30, warmup=5):
     import bench
     eng, diff, cond = bench.build_engine(th.device("cuda", 0), 0, 1)
     if P > 1:  # one text prompt and one image prompt's 16 cutout embeddings (weights as the entry normalises them)
-        D = eng.vit_cfg.output_dim
+        D = eng.towers[0].cfg.output_dim
         del eng, cond  # rebuilt with room for P targets
         th.cuda.empty_cache()
         from clip_guided_diffusion_b200 import guidance as pg

@@ -26,7 +26,7 @@ def _ops(eng):
 def test_one_element_list_engine_is_the_single_tower_engine(monkeypatch):
     ctx = build_tiny("cpu", B=2, cutn=3, image=32, cutn_variants=(2,))
     a = ctx["eng"]
-    b = pg.GuidedStepB200(a.unet.cfg, ctx["ounet"].state_dict(), [a.vit_cfg], [ctx["oclip"].state_dict()], batch=2, num_cutouts=3,
+    b = pg.GuidedStepB200(a.unet.cfg, ctx["ounet"].state_dict(), [a.towers[0].cfg], [ctx["oclip"].state_dict()], batch=2, num_cutouts=3,
                           device="cpu", cutn_variants=(2,), **ctx["kw"])
     assert a.T == b.T == 1 and b.loss_towers is None
     assert _ops(a) == _ops(b) and a.plan.marks == b.plan.marks and a.plan._size == b.plan._size
@@ -146,7 +146,7 @@ def test_fused_steps_consume_the_generator_like_the_towers_make_cutouts():
     th.randn(1, 3, 32, 32)  # the skipped step: the noise only
     assert th.equal(th.get_rng_state(), after)
     assert [tuple(r) for r in eng.v(eng.towers[1].coords, (2, 3)).tolist()] == w[1]
-    assert [tuple(r) for r in eng.v(eng.coords, (2, 3)).tolist()] == w[0]
+    assert [tuple(r) for r in eng.v(eng.towers[0].coords, (2, 3)).tolist()] == w[0]
 
 
 # ---------------------------------------------------------------------------------------------------------------- the entry

@@ -1,7 +1,6 @@
 """GPU: several CLIP towers guiding one step.  CUTOUTS_BWD flags 2 (add into dx) bit for bit on both kernels, the tiny two-tower step
 against the fp32 ensemble oracle (eager and replayed from the CUDA graph), one full-size 256x256 step with ViT-B/32 + ViT-B/16 + RN50
 against the oracle with TF32 off, and the entry end to end with two towers and device-encoded text prompts."""
-import ctypes
 import os
 import unittest.mock as mock
 
@@ -27,15 +26,8 @@ pytestmark = pytest.mark.gpu
 
 # ---------------------------------------------------------------- CUTOUTS_BWD flags 2
 def _cut_bwd(dp, coords, dx, B, H, W, cutn, cs, P, kpad, flags):
-    op = _lib.CgdOp()
-    op.code, op.flags = _lib.OP["CUTOUTS_BWD"], flags
-    for j, v in enumerate([B, H, W, cutn, cs, P, kpad]):
-        op.i[j] = v
-    for j, v in enumerate([0.0, 0.0, 0.0, 0.26862954, 0.26130258, 0.27577711, 0.37]):
-        op.f[j] = v
-    for j, t in enumerate([dp, coords, dx]):
-        op.p[j] = t.data_ptr()
-    _lib.check(_lib.load().cgd_run_op(ctypes.byref(op), ctypes.c_void_p(th.cuda.current_stream().cuda_stream)), "cutouts_bwd")
+    _lib.run_op("CUTOUTS_BWD", flags=flags, i=[B, H, W, cutn, cs, P, kpad], f=[0.0, 0.0, 0.0, 0.26862954, 0.26130258, 0.27577711, 0.37],
+                p=[dp, coords, dx])
 
 
 @pytest.mark.parametrize("B,H,W,cutn,cs,P", [(2, 64, 64, 16, 32, 16),     # row-per-block kernel

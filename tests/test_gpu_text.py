@@ -2,7 +2,6 @@
 TOKEN_EMBED / ROW_GATHER against torch indexing, the text towers of widths 512 / 640 / 768 against the fp32 oracle, and
 ``clip_guided_diffusion(prompts=..., text_encoder="device")`` end to end.  Optional checks against the published vocabulary file and
 the ``clip`` package run when those are present."""
-import ctypes
 import os
 
 import pytest
@@ -25,18 +24,6 @@ pytestmark = pytest.mark.gpu
 gpu_harness.OUT_PTRS.update({"TOKEN_EMBED": [3], "ROW_GATHER": [2]})
 
 
-def _run_op(code, i, p, f=(), flags=0):
-    op = _lib.CgdOp()
-    op.code, op.flags = _lib.OP[code], flags
-    for j, v in enumerate(i):
-        op.i[j] = int(v)
-    for j, v in enumerate(f):
-        op.f[j] = float(v)
-    for j, t in enumerate(p):
-        op.p[j] = t.data_ptr()
-    _lib.check(_lib.load().cgd_run_op(ctypes.byref(op), ctypes.c_void_p(th.cuda.current_stream().cuda_stream)), code.lower())
-
-
 # ---------------------------------------------------------------- causal attention
 def _causal(B, heads, T, d, seed):
     C = heads * d
@@ -44,7 +31,7 @@ def _causal(B, heads, T, d, seed):
     qkv = th.randn(B, T, 3 * C, generator=g).half().cuda()
     out = th.full((B, T, C), float("nan"), dtype=th.float16, device="cuda")
     lse = th.empty(B, heads, T, device="cuda")
-    _run_op("ATTN_FWD", [B, heads, T, d, T * 3 * C, 3 * C, d, T * C, C, d], [qkv, qkv[..., C:], qkv[..., 2 * C:], out, lse], f=[d ** -0.5],
+    _lib.run_op("ATTN_FWD", i=[B, heads, T, d, T * 3 * C, 3 * C, d, T * C, C, d], p=[qkv, qkv[..., C:], qkv[..., 2 * C:], out, lse], f=[d ** -0.5],
             flags=1)
     q, k, v = (t.float().view(B, T, heads, d).transpose(1, 2) for t in qkv.split(C, dim=-1))
     ref = F.scaled_dot_product_attention(q, k, v, is_causal=True).transpose(1, 2).reshape(B, T, C)
@@ -77,7 +64,7 @@ def test_non_causal_attention_is_unchanged_by_the_flag_path():
     qkv = th.randn(B, T, 3 * C, generator=th.Generator().manual_seed(1)).half().cuda()
     out = th.empty(B, T, C, dtype=th.float16, device="cuda")
     lse = th.empty(B, heads, T, device="cuda")
-    _run_op("ATTN_FWD", [B, heads, T, d, T * 3 * C, 3 * C, d, T * C, C, d], [qkv, qkv[..., C:], qkv[..., 2 * C:], out, lse], f=[d ** -0.5])
+    _lib.run_op("ATTN_FWD", i=[B, heads, T, d, T * 3 * C, 3 * C, d, T * C, C, d], p=[qkv, qkv[..., C:], qkv[..., 2 * C:], out, lse], f=[d ** -0.5])
     q, k, v = (t.float().view(B, T, heads, d).transpose(1, 2) for t in qkv.split(C, dim=-1))
     ref = F.scaled_dot_product_attention(q, k, v).transpose(1, 2).reshape(B, T, C)
     assert float((out.float() - ref).abs().max()) <= 4e-3 * float(ref.abs().max())
@@ -91,10 +78,10 @@ def test_token_embed_is_exact(n, T, w, V):
     table = th.randn(V, w, generator=g).half()
     pos = th.randn(T, w, generator=g) * 0.1
     x = th.empty(n, T, w, dtype=th.float16, device="cuda")
-    _run_op("TOKEN_EMBED", [n, T, w, V], [ids.cuda(), table.cuda(), pos.cuda(), x])
+    _lib.run_op("TOKEN_EMBED", i=[n, T, w, V], p=[ids.cuda(), table.cuda(), pos.cuda(), x])
     assert th.equal(x.cpu(), (table.float()[ids.long()] + pos).half())
     ids[0, 1], ids[-1, -1] = V, -3  # outside the table: NaN rows, nothing read outside it
-    _run_op("TOKEN_EMBED", [n, T, w, V], [ids.cuda(), table.cuda(), pos.cuda(), x])
+    _lib.run_op("TOKEN_EMBED", i=[n, T, w, V], p=[ids.cuda(), table.cuda(), pos.cuda(), x])
     got = x.cpu()
     assert got[0, 1].isnan().all() and got[-1, -1].isnan().all() and th.isfinite(got[0, 0]).all()
 
@@ -105,10 +92,10 @@ def test_row_gather_is_exact(rows, w, ldx, ldy, n_src):
     x = th.randn(n_src, ldx, generator=g).half()
     idx = th.randint(0, n_src, (rows,), generator=g, dtype=th.int32)
     y = th.zeros(rows, ldy, dtype=th.float16, device="cuda")
-    _run_op("ROW_GATHER", [rows, w, ldx, ldy, n_src], [x.cuda(), idx.cuda(), y])
+    _lib.run_op("ROW_GATHER", i=[rows, w, ldx, ldy, n_src], p=[x.cuda(), idx.cuda(), y])
     assert th.equal(y.cpu()[:, :w], x[idx.long(), :w]) and not y.cpu()[:, w:].any()
     idx[0] = n_src
-    _run_op("ROW_GATHER", [rows, w, ldx, ldy, n_src], [x.cuda(), idx.cuda(), y])
+    _lib.run_op("ROW_GATHER", i=[rows, w, ldx, ldy, n_src], p=[x.cuda(), idx.cuda(), y])
     assert y.cpu()[0, :w].isnan().all()
 
 
