@@ -13,7 +13,10 @@
 // warpgroups, each issuing wgmma.m64nBNk16 x4 per stage for its 64 pixel rows and accumulating in
 // registers.  Pipeline: STAGES-deep smem ring with full/empty mbarriers; a stage is released once
 // the wgmma group that read it has retired (wait_group 1 keeps one group in flight).
-// Epilogue: the accumulators go to an fp32 staging tile that reuses the ring; then each consumer thread
+// Launches without split-K that write fp16 channel-contiguous outputs (every wide UNet / ViT layer) run the persistent variant
+// `conv_tc_persistent_kernel`: one CTA per SM walks its tiles with the ring carried over, and its epilogue goes through per-warp
+// fp16 sub-tiles outside the ring, so the producer loads the next tile while the consumers finish the last one.
+// conv_tc_kernel's epilogue: the accumulators go to an fp32 staging tile that reuses the ring; then each consumer thread
 // owns one pixel row and half of the tile's channels and adds bias / residual, stores fp16 / fp32 (split-K:
 // one 8-channel chunk of a row per pass, neighbouring threads on neighbouring chunks).
 // Small-M layers (8x8 .. 32x32 feature maps, long-K Linears) split K over gridDim.z: either into an
@@ -51,6 +54,82 @@ struct TcCfg {
   static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 };
 
+// Origin (w0, h0, n0) in the image grid of pixel tile mt.
+__device__ __forceinline__ void tile_origin(const ConvTcParams& p, int mt, int& w0, int& h0, int& n0) {
+  const int tw_i = mt % p.tiles_w;
+  const int th_i = (mt / p.tiles_w) % p.tiles_h;
+  const int tn_i = mt / (p.tiles_w * p.tiles_h);
+  w0 = tw_i * p.TW;
+  h0 = th_i * p.TH;
+  n0 = tn_i * p.TN;
+}
+
+// TMA producer, one tile: K-blocks [kb0, kb1) of the pixel tile at (w0, h0, n0) and output columns [ncol0, ncol0 + BN) into the
+// ring.  (stage, phase) is the producer's ring position; it advances and carries over to the next tile.
+template <int BN>
+__device__ __forceinline__ void produce_kblocks(const CUtensorMap* tmA, const CUtensorMap* tmB, uint8_t* smem_a, uint8_t* smem_b,
+                                                uint64_t* full_bar, uint64_t* empty_bar, const ConvTcParams& p, int kb0, int kb1,
+                                                int w0, int h0, int n0, int ncol0, int& stage, uint32_t& phase) {
+  using Cfg = TcCfg<BN>;
+  const int cblks = p.Cin / BK;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait_trap(&empty_bar[stage], phase ^ 1);
+    mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+    const int tap = kb / cblks, cb = kb - tap * cblks;
+    int dy = 0, dx = 0;
+    if (p.taps == 9) {
+      dy = tap / 3 - 1;
+      dx = tap % 3 - 1;
+    }
+    tma_load_4d(smem_a + stage * Cfg::kABytes, tmA, &full_bar[stage], cb * BK, w0 + dx, h0 + dy, n0);
+    tma_load_4d(smem_b + stage * Cfg::kBBytes, tmB, &full_bar[stage], kb * BK, ncol0, 0, 0);
+    if (++stage == Cfg::kStages) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+}
+
+// Consumer warpgroup wg, one tile: acc = the sum over K-blocks [kb0, kb1) read from the ring at (stage, phase), which advance.
+// A stage is released once the wgmma group that read it has retired; the last stage is returned unreleased, and every wgmma of
+// the tile has retired on return.
+template <int BN>
+__device__ __forceinline__ int consume_kblocks(float* acc, const uint8_t* smem_a, const uint8_t* smem_b, uint64_t* full_bar,
+                                               uint64_t* empty_bar, int wg, int lane, int kb0, int kb1, int& stage, uint32_t& phase) {
+  using Cfg = TcCfg<BN>;
+  int prev = -1;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait_trap(&full_bar[stage], phase);
+    const uint64_t da = make_wgmma_desc_sw128(smem_u32(smem_a + stage * Cfg::kABytes + wg * 64 * 128));
+    const uint64_t db = make_wgmma_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes));
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k)  // advance 16 elements (32 B) along K inside the 128 B swizzle row: +2 in the (>>4) address field
+      wgmma_f16<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > kb0 || k > 0) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();  // the group of the previous stage has retired: its operands may be overwritten
+    if (prev >= 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    }
+    prev = stage;
+    if (++stage == Cfg::kStages) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int j = 0; j < BN / 2; ++j) wgmma_fence_operand(acc[j]);
+  return prev;
+}
+
+// CONV flags 4: acc * QuickGELU'(u), u = the QuickGELU pre-activation read through the residual path
+__device__ __forceinline__ float qgelu_grad_mul(float a, float u) {
+  const float sg = rcp_ftz(1.f + ex2_ftz(-1.702f * 1.4426950408889634f * u));  // sigmoid(1.702 u), MUFU ex2 + rcp
+  return a * (sg * fmaf(1.702f * u, 1.f - sg, 1.f));
+}
+
 template <int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvTcParams p) {
@@ -67,10 +146,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
   // ---- tile coordinates
   const int mt = blockIdx.x;
-  const int tw_i = mt % p.tiles_w;
-  const int th_i = (mt / p.tiles_w) % p.tiles_h;
-  const int tn_i = mt / (p.tiles_w * p.tiles_h);
-  const int w0 = tw_i * p.TW, h0 = th_i * p.TH, n0 = tn_i * p.TN;
+  int w0, h0, n0;
+  tile_origin(p, mt, w0, h0, n0);
   const int ncol0 = blockIdx.y * BN;
   const int kb0 = blockIdx.z * p.kb_per_split;
   const int kb1 = min(kb0 + p.kb_per_split, p.kblocks);  // non-empty for every split (host)
@@ -91,25 +168,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp == kConsumers / 32) {
     // ===== TMA producer
     if (lane == 0) {
-      const int cblks = p.Cin / BK;
       int stage = 0;
       uint32_t phase = 0;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait_trap(&empty_bar[stage], phase ^ 1);
-        mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-        const int tap = kb / cblks, cb = kb - tap * cblks;
-        int dy = 0, dx = 0;
-        if (p.taps == 9) {
-          dy = tap / 3 - 1;
-          dx = tap % 3 - 1;
-        }
-        tma_load_4d(smem_a + stage * Cfg::kABytes, &tmA, &full_bar[stage], cb * BK, w0 + dx, h0 + dy, n0);
-        tma_load_4d(smem_b + stage * Cfg::kBBytes, &tmB, &full_bar[stage], kb * BK, ncol0, 0, 0);
-        if (++stage == Cfg::kStages) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
+      produce_kblocks<BN>(&tmA, &tmB, smem_a, smem_b, full_bar, empty_bar, p, kb0, kb1, w0, h0, n0, ncol0, stage, phase);
     } else if (p.pf_bytes > 0) {
       l2_prefetch_slice(p.pf_ptr, p.pf_bytes, (int)(blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z)),
                         (int)(gridDim.x * gridDim.y * gridDim.z), lane - 1, 31);
@@ -120,31 +181,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     float acc[BN / 2];
 #pragma unroll
     for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
-    int stage = 0, prev = -1;
+    int stage = 0;
     uint32_t phase = 0;
-    for (int kb = kb0; kb < kb1; ++kb) {
-      mbar_wait_trap(&full_bar[stage], phase);
-      const uint64_t da = make_wgmma_desc_sw128(smem_u32(smem_a + stage * Cfg::kABytes + wg * 64 * 128));
-      const uint64_t db = make_wgmma_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes));
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < BK / 16; ++k)  // advance 16 elements (32 B) along K inside the 128 B swizzle row: +2 in the (>>4) address field
-        wgmma_f16<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > kb0 || k > 0) ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<1>();  // the group of the previous stage has retired: its operands may be overwritten
-      if (prev >= 0) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[prev]);
-      }
-      prev = stage;
-      if (++stage == Cfg::kStages) {
-        stage = 0;
-        phase ^= 1;
-      }
-    }
-    wgmma_wait<0>();
-#pragma unroll
-    for (int j = 0; j < BN / 2; ++j) wgmma_fence_operand(acc[j]);
+    consume_kblocks<BN>(acc, smem_a, smem_b, full_bar, empty_bar, wg, lane, kb0, kb1, stage, phase);
     named_bar_sync(1, kConsumers);  // both warpgroups are done reading the ring: it becomes the staging tile
     const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), col0 = 2 * (lane & 3);
 #pragma unroll
@@ -211,12 +250,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           if (p.res) {
             float rr[8];
             unpack8(ld8(p.res + r_off + col), rr);
-            if (p.res_mode == 1) {  // CONV flags 4: out = acc * QuickGELU'(u), u = the tile read through the residual path
+            if (p.res_mode == 1) {
 #pragma unroll
-              for (int e = 0; e < 8; ++e) {
-                const float sg = rcp_ftz(1.f + ex2_ftz(-1.702f * 1.4426950408889634f * rr[e]));  // sigmoid(1.702 u), MUFU ex2 + rcp
-                a[e] *= sg * fmaf(1.702f * rr[e], 1.f - sg, 1.f);
-              }
+              for (int e = 0; e < 8; ++e) a[e] = qgelu_grad_mul(a[e], rr[e]);
             } else {
 #pragma unroll
               for (int e = 0; e < 8; ++e) a[e] += rr[e];
@@ -249,7 +285,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     } else {
       // thread = (pixel row r, half of the columns): measured faster than the chunk mapping above on the one-CTA 256 x 256 layers,
-      // and the coalesced order for channel-strided (NCHW fp32) outputs
+      // and the coalesced order for channel-strided (NCHW fp32) outputs.  Launches that reach it: fp32 or channel-strided outputs
+      // and Cout % 8 != 0; every other one-CTA launch runs conv_tc_persistent_kernel
       const int r = (warp & 3) * 32 + lane, half = warp >> 2;
       const int c_lo = c_base + half * (cw / 2), c_hi = c_lo + cw / 2;
 #pragma unroll 1
@@ -257,6 +294,157 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
   }
   if (p.cluster) cluster_sync_all();  // the other CTAs' reads of this CTA's staging tile are complete before it exits
+}
+
+// ---------------------------------------------------------------- persistent one-CTA kernel
+// The launches without split-K and with an fp16 channel-contiguous output (Cout % 8 == 0): grid = min(tiles, SMs), CTA b owns the
+// tiles b, b + gridDim.x, ... of the (pixel tile, column tile) sequence, pixel tiles fastest.  The producer runs straight on into
+// the next tile's K-blocks; ring stage and phase carry over.  The consumers' K loop is conv_tc_kernel's; their epilogue leaves the
+// ring alone, so the producer refills it meanwhile: bias, then residual or QuickGELU' in fp32 registers (the same operations in the
+// same order as conv_tc_kernel), one rounding to fp16, and per warp two private 16-row x 32-column fp16 sub-tiles in shared memory
+// turn the accumulator fragments into 16-byte row chunks for coalesced residual loads and stores (the residual of the next 32
+// columns is in flight while the current ones are finished).  Results are bitwise those of conv_tc_kernel.
+template <int BN>
+struct PersistCfg {
+  using Ring = TcCfg<BN>;
+  static constexpr int kSubCols = BN < 32 ? BN : 32;  // columns of one epilogue sub-tile (64 needs more registers than BN = 256 has)
+  static constexpr int kChunks = kSubCols / 8;        // 16-byte chunks per sub-tile row
+  static constexpr int kSubLd = kSubCols * 2 + 16;    // bytes per sub-tile row: 16-byte aligned, rows 20 / 12 banks apart
+  static constexpr int kSubBytes = 16 * kSubLd;       // one sub-tile: a consumer warp's 16 rows
+  static constexpr int kPerLane = kChunks / 2;        // chunks per lane and sub-tile in the copy passes
+  static constexpr int kEpiOff = Ring::kStages * Ring::kStageBytes;
+  static constexpr int kBarOff = kEpiOff + (kConsumers / 32) * 2 * kSubBytes;
+  static constexpr int kSmemBytes = kBarOff + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(kPerLane >= 1 && BN % kSubCols == 0, "sub-tile shape");
+  static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
+};
+
+template <int BN>
+__global__ void __launch_bounds__(kThreads, 1)
+conv_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvTcParams p) {
+  using Cfg = PersistCfg<BN>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + Cfg::Ring::kStages * Cfg::Ring::kABytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kBarOff);
+  uint64_t* empty_bar = full_bar + Cfg::Ring::kStages;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m_tiles = p.m_tiles, tiles = p.tiles;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int s = 0; s < Cfg::Ring::kStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], kConsumers / 32);  // one arrive per consumer warp
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (warp == kConsumers / 32) {
+    // ===== TMA producer
+    if (lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+        int w0, h0, n0;
+        tile_origin(p, t % m_tiles, w0, h0, n0);
+        produce_kblocks<BN>(&tmA, &tmB, smem_a, smem_b, full_bar, empty_bar, p, 0, p.kblocks, w0, h0, n0, (t / m_tiles) * BN, stage, phase);
+      }
+    } else if (p.pf_bytes > 0) {
+      l2_prefetch_slice(p.pf_ptr, p.pf_bytes, (int)blockIdx.x, (int)gridDim.x, lane - 1, 31);
+    }
+  } else {
+    // ===== consumer warpgroup wg: pixel rows [64 wg, 64 wg + 64) of every tile; this warp's rows [16 warp, 16 warp + 16)
+    const int wg = warp >> 2;
+    uint8_t* sub0 = smem + Cfg::kEpiOff + warp * 2 * Cfg::kSubBytes;  // this warp's sub-tiles: pass s uses sub0 + (s & 1) * kSubBytes
+    const int fr = lane >> 2, fc = 2 * (lane & 3);  // accumulator fragment: rows fr, fr + 8, columns fc, fc + 1 of every 8
+    float acc[BN / 2];
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+      const int mt = t % m_tiles, ncol0 = (t / m_tiles) * BN;
+      const int last = consume_kblocks<BN>(acc, smem_a, smem_b, full_bar, empty_bar, wg, lane, 0, p.kblocks, stage, phase);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[last]);
+
+      // copy passes: lane owns sub-tile row lane % 16 (pixel row 16 warp + lane % 16 of the tile) and moves its 16-byte chunk
+      // lane / 16 + 2 i in pass i: the 8 lanes of a shared-memory phase read 8 rows, which fall on 8 different groups of 4 banks
+      int w0, h0, n0;
+      tile_origin(p, mt, w0, h0, n0);
+      const int r = warp * 16 + (lane & 15);
+      const int n = n0 + r / (p.TW * p.TH), h = h0 + (r / p.TW) % p.TH, w = w0 + r % p.TW;
+      const bool row_ok = (n < p.NB) && (h < p.H) && (w < p.W);  // partial edge tiles
+      __half* orow = reinterpret_cast<__half*>(p.out) + ((int64_t)n * p.out_sn + (int64_t)h * p.out_sh + (int64_t)w * p.out_sw);
+      const __half* rrow = p.res ? p.res + ((int64_t)n * p.res_sn + (int64_t)h * p.res_sh + (int64_t)w * p.res_sw) : nullptr;
+      // the residual chunks of pass s go straight into its sub-tile (cp.async: loading them through registers would spill at
+      // BN = 256), one pass ahead
+      auto load_res = [&](int s) {
+        uint8_t* srow = sub0 + (s & 1) * Cfg::kSubBytes + (lane & 15) * Cfg::kSubLd;
+#pragma unroll
+        for (int i = 0; i < Cfg::kPerLane; ++i) {
+          const int ch = (lane >> 4) + 2 * i, col = ncol0 + s * Cfg::kSubCols + 8 * ch;
+          if (row_ok && col < p.Cout) cp_async16(srow + 16 * ch, rrow + col);
+        }
+        cp_async_commit();
+      };
+      if (p.res) load_res(0);
+#pragma unroll
+      for (int s = 0; s < BN / Cfg::kSubCols; ++s) {
+        uint8_t* sub = sub0 + (s & 1) * Cfg::kSubBytes;
+        uint8_t* srow = sub + (lane & 15) * Cfg::kSubLd;
+        if (p.res) {
+          if (s + 1 < BN / Cfg::kSubCols) {
+            load_res(s + 1);  // into the other sub-tile: read out before the end of pass s - 1
+            cp_async_wait<1>();
+          } else {
+            cp_async_wait<0>();
+          }
+          __syncwarp();
+        }
+#pragma unroll
+        for (int jj = 0; jj < Cfg::kChunks; ++jj) {
+          const int j = s * Cfg::kChunks + jj;
+          const int col = ncol0 + 8 * j + fc;
+          if (col < p.Cout) {  // Cout % 8 == 0: an 8-column group is wholly inside or outside
+            float v0 = acc[4 * j], v1 = acc[4 * j + 1], v2 = acc[4 * j + 2], v3 = acc[4 * j + 3];
+            if (p.bias) {
+              const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+              v0 += b.x; v1 += b.y; v2 += b.x; v3 += b.y;
+            }
+            __half2* lo = reinterpret_cast<__half2*>(sub + fr * Cfg::kSubLd + 2 * (8 * jj + fc));
+            __half2* hi = reinterpret_cast<__half2*>(sub + (fr + 8) * Cfg::kSubLd + 2 * (8 * jj + fc));
+            if (p.res) {
+              const float2 u0 = __half22float2(*lo), u1 = __half22float2(*hi);
+              if (p.res_mode == 1) {
+                v0 = qgelu_grad_mul(v0, u0.x); v1 = qgelu_grad_mul(v1, u0.y);
+                v2 = qgelu_grad_mul(v2, u1.x); v3 = qgelu_grad_mul(v3, u1.y);
+              } else {
+                v0 += u0.x; v1 += u0.y; v2 += u1.x; v3 += u1.y;
+              }
+            }
+            *lo = __floats2half2_rn(v0, v1);
+            *hi = __floats2half2_rn(v2, v3);
+          }
+        }
+        __syncwarp();
+#pragma unroll
+        for (int i = 0; i < Cfg::kPerLane; ++i) {
+          const int ch = (lane >> 4) + 2 * i, col = ncol0 + s * Cfg::kSubCols + 8 * ch;
+          if (row_ok && col < p.Cout) *reinterpret_cast<uint4*>(orow + col) = *reinterpret_cast<const uint4*>(srow + 16 * ch);
+        }
+        __syncwarp();  // the sub-tile is read out before pass s + 2 (or the next tile) writes it
+      }
+    }
+  }
+  // every store of this CTA has been issued: a dependent launch may take the SM
+  pdl_launch_dependents();
 }
 
 // split-K second pass: sum partials, add bias / residual, store.  One thread per 4 consecutive columns (float4 partial
@@ -433,6 +621,8 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
   p.cluster = 0;
   L.BN = (int)BN;
   L.impl = (int)op.i[18];
+  L.narrow = 0;
+  L.persistent = 0;
   L.A = reinterpret_cast<const __half*>(op.p[0]);
   L.Wp = reinterpret_cast<const __half*>(op.p[1]);
   L.a_sn = op.i[7]; L.a_sh = op.i[8]; L.a_sw = op.i[9];
@@ -440,6 +630,8 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
   L.m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
   p.ws_rows = L.m_tiles * BM;
   L.n_tiles = (int)(Npad / BN);
+  p.m_tiles = L.m_tiles;
+  p.tiles = L.m_tiles * L.n_tiles;
   if (L.impl == 1) return 0;
 
   PFN_encodeTiled enc = get_encode_fn();
@@ -491,6 +683,7 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
     }
     L.narrow = (narrow_on && conv_narrow_eligible(L)) ? 1 : 0;
   }
+  L.persistent = (!L.narrow && p.splits == 1 && !p.cluster && !p.out_f32 && p.out_sc == 1 && p.Cout % 8 == 0) ? 1 : 0;
   return 0;
 }
 
@@ -499,6 +692,7 @@ static int set_smem_attr() {
   static DeviceOnce attr_set;
   if (attr_set.needed()) {
     CGD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BN>::kSmemBytes));
+    CGD_CUDA(cudaFuncSetAttribute(conv_tc_persistent_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, PersistCfg<BN>::kSmemBytes));
     attr_set.mark();
   }
   return 0;
@@ -506,12 +700,16 @@ static int set_smem_attr() {
 
 template <int BN>
 static int launch_tc(const ConvTcLaunch& L, cudaStream_t st) {
-  using Cfg = TcCfg<BN>;
   if (const int rc = set_smem_attr<BN>()) return rc;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)L.m_tiles, (unsigned)L.n_tiles, (unsigned)L.p.splits);
+  if (L.persistent) {
+    cfg.gridDim = dim3((unsigned)std::min(L.m_tiles * L.n_tiles, device_sm_count()));
+    cfg.dynamicSmemBytes = PersistCfg<BN>::kSmemBytes;
+  } else {
+    cfg.gridDim = dim3((unsigned)L.m_tiles, (unsigned)L.n_tiles, (unsigned)L.p.splits);
+    cfg.dynamicSmemBytes = TcCfg<BN>::kSmemBytes;
+  }
   cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
   cfg.stream = st;
   cudaLaunchAttribute attrs[2];
   int na = 0;
@@ -529,7 +727,7 @@ static int launch_tc(const ConvTcLaunch& L, cudaStream_t st) {
   }
   cfg.attrs = attrs;
   cfg.numAttrs = na;
-  CGD_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN>, L.tmA, L.tmB, L.p));
+  CGD_CUDA(cudaLaunchKernelEx(&cfg, L.persistent ? conv_tc_persistent_kernel<BN> : conv_tc_kernel<BN>, L.tmA, L.tmB, L.p));
   return 0;
 }
 

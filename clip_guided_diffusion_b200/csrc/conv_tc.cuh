@@ -12,6 +12,7 @@ struct ConvTcParams {
   int NB, H, W, Cin, Cout, Npad, taps;
   int TW, TH, TN;                    // 128-pixel tile = TW x TH x TN box of the (W, H, N) grid
   int tiles_w, tiles_h, tiles_n;
+  int m_tiles, tiles;                // pixel tiles (tiles_w * tiles_h * tiles_n); output tiles (m_tiles * Npad / BN)
   int kblocks, splits, kb_per_split; // K loop = taps * Cin/64 blocks, optionally split over gridDim.z
   int out_f32;
   int ws_rows;                       // rows per split in the split-K workspace (= m_tiles * 128)
@@ -34,6 +35,7 @@ struct ConvTcLaunch {
   ConvTcParams p;
   int BN, impl, m_tiles, n_tiles;
   int narrow;                        // <= 8 output channels, fp32 out, 3x3: the halo-tile mma.sync kernel of conv_narrow.cu instead of a wgmma tile
+  int persistent;                    // no split-K, fp16 channel-contiguous out, Cout % 8 == 0: conv_tc_persistent_kernel (min(tiles, SMs) CTAs)
   const __half* A;
   const __half* Wp;
   int64_t a_sn, a_sh, a_sw;

@@ -74,6 +74,14 @@ __device__ __forceinline__ void l2_prefetch_slice(const void* ptr, int64_t bytes
   if (hi > lo)
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<const char*>(ptr) + lo), "r"((uint32_t)(hi - lo)) : "memory");
 }
+// 16-byte asynchronous copy global -> shared (no register staging), committed in groups; cp_async_wait<N>() returns once at
+// most N of this thread's groups are pending
+__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem)), "l"(gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
