@@ -14,8 +14,9 @@
 // registers.  Pipeline: STAGES-deep smem ring with full/empty mbarriers; a stage is released once
 // the wgmma group that read it has retired (wait_group 1 keeps one group in flight).
 // Launches without split-K that write fp16 channel-contiguous outputs (every wide UNet / ViT layer) run the persistent variant
-// `conv_tc_persistent_kernel`: one CTA per SM walks its tiles with the ring carried over, and its epilogue goes through per-warp
-// fp16 sub-tiles outside the ring, so the producer loads the next tile while the consumers finish the last one.
+// `conv_tc_persistent_kernel`: one CTA per SM walks its tiles with the ring carried over; its epilogue goes through an fp16 staging
+// tile outside the ring that the TMA unit fills with the residual during the K loop and stores from, so the producer loads the
+// next tile while the consumers finish the last one, and the consumers do not wait for their stores.
 // conv_tc_kernel's epilogue: the accumulators go to an fp32 staging tile that reuses the ring; then each consumer thread
 // owns one pixel row and half of the tile's channels and adds bias / residual, stores fp16 / fp32 (split-K:
 // one 8-channel chunk of a row per pass, neighbouring threads on neighbouring chunks).
@@ -54,6 +55,26 @@ struct TcCfg {
   static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 };
 
+// Phase stamps of conv_tc_persistent_kernel, compiled in only with -DCGD_CONV_PHASES (scripts/conv_tile_phases.py builds that
+// variant; the default build has none of it).  Per CTA and tile slot, %globaltimer ns: [0] consumer thread 0 enters the tile's
+// K loop, [1] its first full-barrier pass, [2] the end of its K loop (after wgmma wait_group 0), [3] the end of its epilogue,
+// [4] the producer's time blocked on empty barriers while loading the tile.  Later launches overwrite earlier ones.
+#ifdef CGD_CONV_PHASES
+constexpr int kPhaseCtas = 256, kPhaseTiles = 32, kPhaseFields = 5;
+__device__ unsigned long long g_conv_phases[kPhaseCtas * kPhaseTiles * kPhaseFields];
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ void phase_stamp(int slot, int field, unsigned long long v) {
+  if (blockIdx.x < kPhaseCtas && slot < kPhaseTiles) g_conv_phases[(blockIdx.x * kPhaseTiles + slot) * kPhaseFields + field] = v;
+}
+#define CGD_PHASE(...) __VA_ARGS__
+#else
+#define CGD_PHASE(...)
+#endif
+
 // Origin (w0, h0, n0) in the image grid of pixel tile mt.
 __device__ __forceinline__ void tile_origin(const ConvTcParams& p, int mt, int& w0, int& h0, int& n0) {
   const int tw_i = mt % p.tiles_w;
@@ -65,15 +86,19 @@ __device__ __forceinline__ void tile_origin(const ConvTcParams& p, int mt, int& 
 }
 
 // TMA producer, one tile: K-blocks [kb0, kb1) of the pixel tile at (w0, h0, n0) and output columns [ncol0, ncol0 + BN) into the
-// ring.  (stage, phase) is the producer's ring position; it advances and carries over to the next tile.
-template <int BN>
-__device__ __forceinline__ void produce_kblocks(const CUtensorMap* tmA, const CUtensorMap* tmB, uint8_t* smem_a, uint8_t* smem_b,
-                                                uint64_t* full_bar, uint64_t* empty_bar, const ConvTcParams& p, int kb0, int kb1,
-                                                int w0, int h0, int n0, int ncol0, int& stage, uint32_t& phase) {
+// ring.  (stage, phase) is the producer's ring position; it advances and carries over to the next tile.  Returns the ns spent
+// blocked on empty barriers under CGD_CONV_PHASES, else 0.
+template <int BN, int STAGES = TcCfg<BN>::kStages>
+__device__ __forceinline__ unsigned long long produce_kblocks(const CUtensorMap* tmA, const CUtensorMap* tmB, uint8_t* smem_a, uint8_t* smem_b,
+                                                              uint64_t* full_bar, uint64_t* empty_bar, const ConvTcParams& p, int kb0, int kb1,
+                                                              int w0, int h0, int n0, int ncol0, int& stage, uint32_t& phase) {
   using Cfg = TcCfg<BN>;
   const int cblks = p.Cin / BK;
+  unsigned long long blocked = 0;
   for (int kb = kb0; kb < kb1; ++kb) {
+    CGD_PHASE(const unsigned long long tw = globaltimer_ns();)
     mbar_wait_trap(&empty_bar[stage], phase ^ 1);
+    CGD_PHASE(blocked += globaltimer_ns() - tw;)
     mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
     const int tap = kb / cblks, cb = kb - tap * cblks;
     int dy = 0, dx = 0;
@@ -83,19 +108,21 @@ __device__ __forceinline__ void produce_kblocks(const CUtensorMap* tmA, const CU
     }
     tma_load_4d(smem_a + stage * Cfg::kABytes, tmA, &full_bar[stage], cb * BK, w0 + dx, h0 + dy, n0);
     tma_load_4d(smem_b + stage * Cfg::kBBytes, tmB, &full_bar[stage], kb * BK, ncol0, 0, 0);
-    if (++stage == Cfg::kStages) {
+    if (++stage == STAGES) {
       stage = 0;
       phase ^= 1;
     }
   }
+  return blocked;
 }
 
 // Consumer warpgroup wg, one tile: acc = the sum over K-blocks [kb0, kb1) read from the ring at (stage, phase), which advance.
 // A stage is released once the wgmma group that read it has retired; the last stage is returned unreleased, and every wgmma of
-// the tile has retired on return.
-template <int BN>
+// the tile has retired on return.  after_first() runs once the first K-block's wgmma group has been issued.
+template <int BN, int STAGES = TcCfg<BN>::kStages, class AfterFirst>
 __device__ __forceinline__ int consume_kblocks(float* acc, const uint8_t* smem_a, const uint8_t* smem_b, uint64_t* full_bar,
-                                               uint64_t* empty_bar, int wg, int lane, int kb0, int kb1, int& stage, uint32_t& phase) {
+                                               uint64_t* empty_bar, int wg, int lane, int kb0, int kb1, int& stage, uint32_t& phase,
+                                               AfterFirst after_first) {
   using Cfg = TcCfg<BN>;
   int prev = -1;
   for (int kb = kb0; kb < kb1; ++kb) {
@@ -107,13 +134,14 @@ __device__ __forceinline__ int consume_kblocks(float* acc, const uint8_t* smem_a
     for (int k = 0; k < BK / 16; ++k)  // advance 16 elements (32 B) along K inside the 128 B swizzle row: +2 in the (>>4) address field
       wgmma_f16<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > kb0 || k > 0) ? 1u : 0u);
     wgmma_commit();
+    if (kb == kb0) after_first();
     wgmma_wait<1>();  // the group of the previous stage has retired: its operands may be overwritten
     if (prev >= 0) {
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
     }
     prev = stage;
-    if (++stage == Cfg::kStages) {
+    if (++stage == STAGES) {
       stage = 0;
       phase ^= 1;
     }
@@ -183,7 +211,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
     int stage = 0;
     uint32_t phase = 0;
-    consume_kblocks<BN>(acc, smem_a, smem_b, full_bar, empty_bar, wg, lane, kb0, kb1, stage, phase);
+    consume_kblocks<BN>(acc, smem_a, smem_b, full_bar, empty_bar, wg, lane, kb0, kb1, stage, phase, [] {});
     named_bar_sync(1, kConsumers);  // both warpgroups are done reading the ring: it becomes the staging tile
     const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), col0 = 2 * (lane & 3);
 #pragma unroll
@@ -299,36 +327,62 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // ---------------------------------------------------------------- persistent one-CTA kernel
 // The launches without split-K and with an fp16 channel-contiguous output (Cout % 8 == 0): grid = min(tiles, SMs), CTA b owns the
 // tiles b, b + gridDim.x, ... of the (pixel tile, column tile) sequence, pixel tiles fastest.  The producer runs straight on into
-// the next tile's K-blocks; ring stage and phase carry over.  The consumers' K loop is conv_tc_kernel's; their epilogue leaves the
-// ring alone, so the producer refills it meanwhile: bias, then residual or QuickGELU' in fp32 registers (the same operations in the
-// same order as conv_tc_kernel), one rounding to fp16, and per warp two private 16-row x 32-column fp16 sub-tiles in shared memory
-// turn the accumulator fragments into 16-byte row chunks for coalesced residual loads and stores (the residual of the next 32
-// columns is in flight while the current ones are finished).  Results are bitwise those of conv_tc_kernel.
+// the next tile's K-blocks; ring stage and phase carry over.  The consumers' K loop is conv_tc_kernel's.  Their epilogue goes
+// through a staging tile outside the ring, so the producer refills the ring meanwhile:
+//   * the staging tile is the 128 x BN fp16 output tile as BN / 64 TMA boxes of 64 channels in the 128-byte-swizzled layout
+//     (narrower boxes and swizzles at BN < 64); at BN 256 it holds one 128-column half at a time, the two halves stored in turn,
+//     the second half's residual loaded by consumer thread 0 once the first half's store has been read out;
+//   * the producer lane TMA-loads a tile's residual into it while the consumers run that tile's K loop, once the previous tile's
+//     store has been read out of it (`stg_free`), and signals `stg_full` (with the transaction bytes; a plain arrive without a
+//     residual);
+//   * the consumers add bias, then residual or QuickGELU' in fp32 registers (the same operations in the same order as
+//     conv_tc_kernel), round once to fp16 and write the result in place; after a named barrier consumer thread 0 TMA-stores the
+//     tile (the TMA unit clips rows outside the image and columns >= Cout) and the consumers go on into the next K loop;
+//   * thread 0 waits for that store to be read out of shared memory after issuing the next tile's first wgmma group, then
+//     arrives on `stg_free`; it drains its stores before the CTA exits.
+// Results are bitwise those of conv_tc_kernel.
 template <int BN>
 struct PersistCfg {
   using Ring = TcCfg<BN>;
-  static constexpr int kSubCols = BN < 32 ? BN : 32;  // columns of one epilogue sub-tile (64 needs more registers than BN = 256 has)
-  static constexpr int kChunks = kSubCols / 8;        // 16-byte chunks per sub-tile row
-  static constexpr int kSubLd = kSubCols * 2 + 16;    // bytes per sub-tile row: 16-byte aligned, rows 20 / 12 banks apart
-  static constexpr int kSubBytes = 16 * kSubLd;       // one sub-tile: a consumer warp's 16 rows
-  static constexpr int kPerLane = kChunks / 2;        // chunks per lane and sub-tile in the copy passes
-  static constexpr int kEpiOff = Ring::kStages * Ring::kStageBytes;
-  static constexpr int kBarOff = kEpiOff + (kConsumers / 32) * 2 * kSubBytes;
+  static constexpr int kStages = Ring::kStages;
+  // at BN 256 four 48 KB stages and a 64 KB staging tile exceed 227 KB: the staging tile holds one 128-column half at a time (measured
+  // against a 3-stage ring with the whole tile staged: DESIGN §4)
+  static constexpr int kHalves = BN == 256 ? 2 : 1;
+  static constexpr int kBoxC = BN < 64 ? BN : 64;                // channels per staging box: one 128-byte swizzle row at BN >= 64
+  static constexpr int kRowBytes = kBoxC * 2;
+  static constexpr int kSwMask = kRowBytes / 16 - 1;             // swizzle span 128 / 64 / 32 bytes: XOR of 3 / 2 / 1 chunk-index bits
+  static constexpr int kBoxBytes = BM * kRowBytes;
+  static constexpr int kBoxes = BN / kBoxC;
+  static constexpr int kStgOff = kStages * Ring::kStageBytes;    // a multiple of 1024: the swizzle pattern's alignment
+  static constexpr int kStgBoxes = kBoxes / kHalves;
+  static constexpr int kBiasOff = kStgOff + kStgBoxes * kBoxBytes;
+  static constexpr int kBarOff = kBiasOff + BN * 4;
   static constexpr int kSmemBytes = kBarOff + 1024 /*align slack*/ + 256 /*barriers*/;
-  static_assert(kPerLane >= 1 && BN % kSubCols == 0, "sub-tile shape");
+  static_assert(kStgOff % 1024 == 0 && kBoxBytes % 1024 == 0, "staging boxes must start on a 1024-byte boundary");
   static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
+  // byte offset of (row r, byte b of the row) in a staging box: the TMA unit's swizzle (16-byte chunk index ^= bits 7.. of the offset)
+  static __device__ __forceinline__ int swz(int r, int b) {
+    const int off = r * kRowBytes + b;
+    return off ^ (((off >> 7) & kSwMask) << 4);
+  }
 };
 
 template <int BN>
 __global__ void __launch_bounds__(kThreads, 1)
-conv_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvTcParams p) {
+conv_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                          const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmRes, const ConvTcParams p) {
   using Cfg = PersistCfg<BN>;
+  constexpr int S = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + Cfg::Ring::kStages * Cfg::Ring::kABytes;
+  uint8_t* smem_b = smem + S * Cfg::Ring::kABytes;
+  uint8_t* stg = smem + Cfg::kStgOff;
+  float* bias_s = reinterpret_cast<float*>(smem + Cfg::kBiasOff);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kBarOff);
-  uint64_t* empty_bar = full_bar + Cfg::Ring::kStages;
+  uint64_t* empty_bar = full_bar + S;
+  uint64_t* stg_free = empty_bar + S;  // the previous tile's store has been read out of the staging tile
+  uint64_t* stg_full = stg_free + 1;   // the staging tile holds this tile's residual (or is merely free, without one)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_tiles = p.m_tiles, tiles = p.tiles;
@@ -336,10 +390,14 @@ conv_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int s = 0; s < Cfg::Ring::kStages; ++s) {
+    tma_prefetch_desc(&tmOut);
+    if (p.res) tma_prefetch_desc(&tmRes);
+    for (int s = 0; s < S; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], kConsumers / 32);  // one arrive per consumer warp
     }
+    mbar_init(stg_free, 1);
+    mbar_init(stg_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -350,76 +408,101 @@ conv_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+      // the residual goes in from the end of the first ring-full of K-blocks: by then the consumers are in this tile's K loop, so the
+      // previous tile's store is issued.  Its boxes are spread over the rest of the K loop, one every `step` K-blocks, so that they
+      // do not arrive in one burst on top of the operand loads
+      const int kres = min(S, p.kblocks);
+      for (int t = blockIdx.x, i = 0; t < tiles; t += gridDim.x, ++i) {
         int w0, h0, n0;
         tile_origin(p, t % m_tiles, w0, h0, n0);
-        produce_kblocks<BN>(&tmA, &tmB, smem_a, smem_b, full_bar, empty_bar, p, 0, p.kblocks, w0, h0, n0, (t / m_tiles) * BN, stage, phase);
+        const int ncol0 = (t / m_tiles) * BN;
+        unsigned long long blocked =
+            produce_kblocks<BN, S>(&tmA, &tmB, smem_a, smem_b, full_bar, empty_bar, p, 0, kres, w0, h0, n0, ncol0, stage, phase);
+        if (i > 0) mbar_wait_trap(stg_free, (i - 1) & 1);
+        int kb = kres;
+        // boxes wholly beyond Cout are skipped (a column tile may lie wholly beyond it when Npad - Cout >= BN)
+        const int nb = max(0, min(Cfg::kStgBoxes, (p.Cout - ncol0 + Cfg::kBoxC - 1) / Cfg::kBoxC));
+        if (p.res && nb > 0) {
+          const int step = (p.kblocks - kres) / nb;
+          mbar_expect_tx(stg_full, nb * Cfg::kBoxBytes);
+          for (int b = 0; b < nb; ++b) {
+            const int kb_next = kres + b * step;
+            blocked += produce_kblocks<BN, S>(&tmA, &tmB, smem_a, smem_b, full_bar, empty_bar, p, kb, kb_next, w0, h0, n0, ncol0, stage, phase);
+            kb = kb_next;
+            tma_load_4d(stg + b * Cfg::kBoxBytes, &tmRes, stg_full, ncol0 + b * Cfg::kBoxC, w0, h0, n0);
+          }
+        } else {
+          mbar_arrive(stg_full);
+        }
+        blocked += produce_kblocks<BN, S>(&tmA, &tmB, smem_a, smem_b, full_bar, empty_bar, p, kb, p.kblocks, w0, h0, n0, ncol0, stage, phase);
+        CGD_PHASE(phase_stamp(i, 4, blocked);)
+        (void)blocked;
       }
     } else if (p.pf_bytes > 0) {
       l2_prefetch_slice(p.pf_ptr, p.pf_bytes, (int)blockIdx.x, (int)gridDim.x, lane - 1, 31);
     }
   } else {
-    // ===== consumer warpgroup wg: pixel rows [64 wg, 64 wg + 64) of every tile; this warp's rows [16 warp, 16 warp + 16)
+    // ===== consumer warpgroup wg: pixel rows [64 wg, 64 wg + 64) of every tile; this thread's fragment rows r0 and r0 + 8
     const int wg = warp >> 2;
-    uint8_t* sub0 = smem + Cfg::kEpiOff + warp * 2 * Cfg::kSubBytes;  // this warp's sub-tiles: pass s uses sub0 + (s & 1) * kSubBytes
     const int fr = lane >> 2, fc = 2 * (lane & 3);  // accumulator fragment: rows fr, fr + 8, columns fc, fc + 1 of every 8
+    const int r0 = warp * 16 + fr;
     float acc[BN / 2];
 #pragma unroll
     for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
     int stage = 0;
-    uint32_t phase = 0;
-    for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+    uint32_t phase = 0, sp = 0;
+    for (int t = blockIdx.x, i = 0; t < tiles; t += gridDim.x, ++i) {
       const int mt = t % m_tiles, ncol0 = (t / m_tiles) * BN;
-      const int last = consume_kblocks<BN>(acc, smem_a, smem_b, full_bar, empty_bar, wg, lane, 0, p.kblocks, stage, phase);
+      // this thread's bias column, in flight during the K loop
+      const float bias_v = (p.bias && threadIdx.x < BN && ncol0 + (int)threadIdx.x < p.Cout) ? __ldg(p.bias + ncol0 + threadIdx.x) : 0.f;
+      CGD_PHASE(if (threadIdx.x == 0) phase_stamp(i, 0, globaltimer_ns());)
+      const int last = consume_kblocks<BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, wg, lane, 0, p.kblocks, stage, phase, [&] {
+        CGD_PHASE(if (threadIdx.x == 0) phase_stamp(i, 1, globaltimer_ns());)
+        // the previous tile's store must be read out of the staging tile before the producer may refill it.  Waiting here, with this
+        // tile's first wgmma group in flight, stalls warp 0 (and through its stage releases the producer) only while that read-out
+        // is still running; the phase stamps show no longer operand wait at tile start
+        if (threadIdx.x == 0 && i > 0) {
+          bulk_wait_read<0>();
+          mbar_arrive(stg_free);
+        }
+      });
+      CGD_PHASE(if (threadIdx.x == 0) phase_stamp(i, 2, globaltimer_ns());)
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_bar[last]);
 
-      // copy passes: lane owns sub-tile row lane % 16 (pixel row 16 warp + lane % 16 of the tile) and moves its 16-byte chunk
-      // lane / 16 + 2 i in pass i: the 8 lanes of a shared-memory phase read 8 rows, which fall on 8 different groups of 4 banks
+      if (p.bias) {  // every consumer has finished the previous tile's epilogue (named barrier 1), so bias_s is free
+        if (threadIdx.x < BN) bias_s[threadIdx.x] = bias_v;
+        named_bar_sync(2, kConsumers);
+      }
       int w0, h0, n0;
       tile_origin(p, mt, w0, h0, n0);
-      const int r = warp * 16 + (lane & 15);
-      const int n = n0 + r / (p.TW * p.TH), h = h0 + (r / p.TW) % p.TH, w = w0 + r % p.TW;
-      const bool row_ok = (n < p.NB) && (h < p.H) && (w < p.W);  // partial edge tiles
-      __half* orow = reinterpret_cast<__half*>(p.out) + ((int64_t)n * p.out_sn + (int64_t)h * p.out_sh + (int64_t)w * p.out_sw);
-      const __half* rrow = p.res ? p.res + ((int64_t)n * p.res_sn + (int64_t)h * p.res_sh + (int64_t)w * p.res_sw) : nullptr;
-      // the residual chunks of pass s go straight into its sub-tile (cp.async: loading them through registers would spill at
-      // BN = 256), one pass ahead
-      auto load_res = [&](int s) {
-        uint8_t* srow = sub0 + (s & 1) * Cfg::kSubBytes + (lane & 15) * Cfg::kSubLd;
 #pragma unroll
-        for (int i = 0; i < Cfg::kPerLane; ++i) {
-          const int ch = (lane >> 4) + 2 * i, col = ncol0 + s * Cfg::kSubCols + 8 * ch;
-          if (row_ok && col < p.Cout) cp_async16(srow + 16 * ch, rrow + col);
-        }
-        cp_async_commit();
-      };
-      if (p.res) load_res(0);
-#pragma unroll
-      for (int s = 0; s < BN / Cfg::kSubCols; ++s) {
-        uint8_t* sub = sub0 + (s & 1) * Cfg::kSubBytes;
-        uint8_t* srow = sub + (lane & 15) * Cfg::kSubLd;
-        if (p.res) {
-          if (s + 1 < BN / Cfg::kSubCols) {
-            load_res(s + 1);  // into the other sub-tile: read out before the end of pass s - 1
-            cp_async_wait<1>();
+      for (int h = 0; h < Cfg::kHalves; ++h) {
+        const int bbase = h * Cfg::kStgBoxes;
+        const int nbh = max(0, min(Cfg::kStgBoxes, (p.Cout - ncol0 + Cfg::kBoxC - 1) / Cfg::kBoxC - bbase));
+        if (h > 0 && threadIdx.x == 0) {  // the first half's store must be read out before the second half's residual lands
+          bulk_wait_read<0>();
+          if (p.res && nbh > 0) {
+            mbar_expect_tx(stg_full, nbh * Cfg::kBoxBytes);
+            for (int b = 0; b < nbh; ++b) tma_load_4d(stg + b * Cfg::kBoxBytes, &tmRes, stg_full, ncol0 + (bbase + b) * Cfg::kBoxC, w0, h0, n0);
           } else {
-            cp_async_wait<0>();
+            mbar_arrive(stg_full);
           }
-          __syncwarp();
         }
+        mbar_wait_trap(stg_full, sp);
+        sp ^= 1;
 #pragma unroll
-        for (int jj = 0; jj < Cfg::kChunks; ++jj) {
-          const int j = s * Cfg::kChunks + jj;
-          const int col = ncol0 + 8 * j + fc;
-          if (col < p.Cout) {  // Cout % 8 == 0: an 8-column group is wholly inside or outside
+        for (int j = h * BN / 8 / Cfg::kHalves; j < (h + 1) * BN / 8 / Cfg::kHalves; ++j) {
+          if (ncol0 + 8 * j < p.Cout) {
             float v0 = acc[4 * j], v1 = acc[4 * j + 1], v2 = acc[4 * j + 2], v3 = acc[4 * j + 3];
             if (p.bias) {
-              const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+              const float2 b = *reinterpret_cast<const float2*>(bias_s + 8 * j + fc);
               v0 += b.x; v1 += b.y; v2 += b.x; v3 += b.y;
             }
-            __half2* lo = reinterpret_cast<__half2*>(sub + fr * Cfg::kSubLd + 2 * (8 * jj + fc));
-            __half2* hi = reinterpret_cast<__half2*>(sub + (fr + 8) * Cfg::kSubLd + 2 * (8 * jj + fc));
+            uint8_t* box = stg + (8 * j / Cfg::kBoxC - bbase) * Cfg::kBoxBytes;
+            const int cb = 2 * (8 * j % Cfg::kBoxC + fc);
+            __half2* lo = reinterpret_cast<__half2*>(box + Cfg::swz(r0, cb));
+            __half2* hi = reinterpret_cast<__half2*>(box + Cfg::swz(r0 + 8, cb));
             if (p.res) {
               const float2 u0 = __half22float2(*lo), u1 = __half22float2(*hi);
               if (p.res_mode == 1) {
@@ -433,17 +516,18 @@ conv_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
             *hi = __floats2half2_rn(v2, v3);
           }
         }
-        __syncwarp();
-#pragma unroll
-        for (int i = 0; i < Cfg::kPerLane; ++i) {
-          const int ch = (lane >> 4) + 2 * i, col = ncol0 + s * Cfg::kSubCols + 8 * ch;
-          if (row_ok && col < p.Cout) *reinterpret_cast<uint4*>(orow + col) = *reinterpret_cast<const uint4*>(srow + 16 * ch);
+        fence_proxy_async_smem();  // this half's generic-proxy writes, before the TMA unit reads them
+        named_bar_sync(1, kConsumers);
+        if (threadIdx.x == 0) {
+          for (int b = 0; b < nbh; ++b) tma_store_4d(&tmOut, stg + b * Cfg::kBoxBytes, ncol0 + (bbase + b) * Cfg::kBoxC, w0, h0, n0);
+          bulk_commit();
         }
-        __syncwarp();  // the sub-tile is read out before pass s + 2 (or the next tile) writes it
       }
+      CGD_PHASE(if (threadIdx.x == 0) phase_stamp(i, 3, globaltimer_ns());)
     }
+    if (threadIdx.x == 0) bulk_wait<0>();  // the CTA's stores are complete before its shared memory is released
   }
-  // every store of this CTA has been issued: a dependent launch may take the SM
+  // every store of this CTA has completed: a dependent launch may take the SM
   pdl_launch_dependents();
 }
 
@@ -684,6 +768,28 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
     L.narrow = (narrow_on && conv_narrow_eligible(L)) ? 1 : 0;
   }
   L.persistent = (!L.narrow && p.splits == 1 && !p.cluster && !p.out_f32 && p.out_sc == 1 && p.Cout % 8 == 0) ? 1 : 0;
+  if (L.persistent) {
+    // output / residual boxes of the persistent epilogue: 128 pixels x min(BN, 64) channels, swizzled like the staging tile.  The C
+    // extent is Cout, so the TMA unit clips padded columns and pixels outside the image; channel slices are a base pointer plus
+    // the row strides checked above
+    const cuuint32_t boxc = (cuuint32_t)std::min<int64_t>(BN, 64);
+    const CUtensorMapSwizzle sw = boxc == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : boxc == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
+    auto encode_io = [&](CUtensorMap* tm, const void* ptr, int64_t sn, int64_t sh, int64_t sw_, const char* what) {
+      cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)NB};
+      cuuint64_t strides[3] = {(cuuint64_t)sw_ * 2, (cuuint64_t)sh * 2, (cuuint64_t)sn * 2};
+      cuuint32_t box[4] = {boxc, (cuuint32_t)p.TW, (cuuint32_t)p.TH, (cuuint32_t)p.TN};
+      cuuint32_t estr[4] = {1, 1, 1, 1};
+      CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                       sw, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      CGD_CHECK_ARG(r == CUDA_SUCCESS, "conv: cuTensorMapEncodeTiled(%s) failed with %d (strides %lld,%lld,%lld)", what, (int)r,
+                    (long long)sw_, (long long)sh, (long long)sn);
+      return 0;
+    };
+    if (const int rc = encode_io(&L.tmOut, p.out, p.out_sn, p.out_sh, p.out_sw, "out")) return rc;
+    if (p.res) {
+      if (const int rc = encode_io(&L.tmRes, p.res, p.res_sn, p.res_sh, p.res_sw, "res")) return rc;
+    }
+  }
   return 0;
 }
 
@@ -727,7 +833,8 @@ static int launch_tc(const ConvTcLaunch& L, cudaStream_t st) {
   }
   cfg.attrs = attrs;
   cfg.numAttrs = na;
-  CGD_CUDA(cudaLaunchKernelEx(&cfg, L.persistent ? conv_tc_persistent_kernel<BN> : conv_tc_kernel<BN>, L.tmA, L.tmB, L.p));
+  if (L.persistent) CGD_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_persistent_kernel<BN>, L.tmA, L.tmB, L.tmOut, L.tmRes, L.p));
+  else CGD_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN>, L.tmA, L.tmB, L.p));
   return 0;
 }
 
@@ -803,3 +910,14 @@ int conv_tc_num_launches(const ConvTcLaunch& L) {
 }
 
 }  // namespace cgd
+
+#ifdef CGD_CONV_PHASES
+// The instrumented build only: copies the [kPhaseCtas][kPhaseTiles][kPhaseFields] stamps to `host` (n elements), then zeroes them.
+extern "C" int cgd_conv_phases(unsigned long long* host, int n) {
+  if (n != cgd::kPhaseCtas * cgd::kPhaseTiles * cgd::kPhaseFields) return -1;
+  if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(host, cgd::g_conv_phases, sizeof(cgd::g_conv_phases)) != cudaSuccess)
+    return -1;
+  static unsigned long long zeros[cgd::kPhaseCtas * cgd::kPhaseTiles * cgd::kPhaseFields];
+  return cudaMemcpyToSymbol(cgd::g_conv_phases, zeros, sizeof(zeros)) == cudaSuccess ? 0 : -1;
+}
+#endif

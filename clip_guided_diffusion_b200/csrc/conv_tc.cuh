@@ -32,6 +32,7 @@ struct ConvTcParams {
 
 struct ConvTcLaunch {
   CUtensorMap tmA, tmB;              // A: 4-D pixel box; B: [Npad, K] weights (4-D map, unit outer dims), [BN x 64] weight slice per load
+  CUtensorMap tmOut, tmRes;          // persistent kernel: output / residual (C = Cout, W, H, N), one 128-pixel x 64-channel box per load / store
   ConvTcParams p;
   int BN, impl, m_tiles, n_tiles;
   int narrow;                        // <= 8 output channels, fp32 out, 3x3: the halo-tile mma.sync kernel of conv_narrow.cu instead of a wgmma tile
