@@ -107,9 +107,15 @@ __global__ void gn_stats_kernel(const __half* __restrict__ x, float* __restrict_
   const int cpg = C / 32;
   const int ppc = (HW + nchunk - 1) / nchunk;
   const int p0 = chunk * ppc, p1 = min(HW, p0 + ppc);
-  float s[8], q[8];
+  // sums about a per-group pivot (the group's first element, the same in every block): the fold's E[x^2] - mean^2 then cancels only
+  // over the spread of x around it, not over the group's mean.  That assumes the pivot (pixel 0, an image corner) lies within a few
+  // std of the mean: k std away costs ~log2(1 + k^2) bits, as before; not measured on real activations.
+  float s[8], q[8], piv[8];
 #pragma unroll
-  for (int j = 0; j < 8; ++j) s[j] = q[j] = 0.f;
+  for (int j = 0; j < 8; ++j) {
+    s[j] = q[j] = 0.f;
+    piv[j] = __half2float(x[(int64_t)n * HW * ld + (col * 8 + j) / cpg * cpg]);
+  }
   const __half* xb = x + (int64_t)n * HW * ld + col * 8;
   for (int p = p0 + pl; p < p1; p += 4 * PP) {  // 4 independent 128-bit loads in flight per thread
     half8 raw[4];
@@ -123,8 +129,9 @@ __global__ void gn_stats_kernel(const __half* __restrict__ x, float* __restrict_
         unpack8(raw[u], v);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-          s[j] += v[j];
-          q[j] = fmaf(v[j], v[j], q[j]);
+          const float d = v[j] - piv[j];
+          s[j] += d;
+          q[j] = fmaf(d, d, q[j]);
         }
       }
     }
@@ -146,9 +153,10 @@ __global__ void gn_stats_kernel(const __half* __restrict__ x, float* __restrict_
     if (threadIdx.x < 32) {
       const double ds = fold_s[threadIdx.x], dq = fold_q[threadIdx.x];
       const double m = (double)cpg * (double)HW;
-      const double mean = ds / m;
-      double var = dq / m - mean * mean;
+      const double dm = ds / m;  // mean - pivot
+      double var = dq / m - dm * dm;
       if (var < 0.0) var = 0.0;
+      const double mean = (double)__half2float(x[(int64_t)n * HW * ld + threadIdx.x * cpg]) + dm;
       stats[((int64_t)n * 32 + threadIdx.x) * 2 + 0] = (float)mean;
       stats[((int64_t)n * 32 + threadIdx.x) * 2 + 1] = (float)(1.0 / sqrt(var + (double)eps));
     }

@@ -25,53 +25,7 @@ from clip_guided_diffusion_b200.guidance import CLIP_MEAN, CLIP_STD
 from clip_guided_diffusion_b200.plan import Plan
 from clip_guided_diffusion_b200.rn import RN_CONFIGS
 from clip_guided_diffusion_b200.vit import VIT_CONFIGS
-from tests.ensemble_oracle import EnsembleInterp  # the plan interpreter, with CUTOUTS_BWD flags 2 (accumulate)
-
-U = 2.0 ** -24  # fp32 unit round-off
-D64 = th.float64
-
-
-# ---------------------------------------------------------------------------------------------------------------- harness
-def run(plan, device, inputs):
-    """Finalize `plan` on `device`, write `inputs` ([(Buf, tensor)]) into its arena, execute every op -- the CUDA kernels on "cuda",
-    the test interpreter on "cpu" -- and return a reader Buf -> CPU tensor."""
-    plan.finalize(device)
-    for b, t in inputs:
-        v = plan.view(b)
-        v.copy_(t.reshape(-1).to(v.dtype))
-    if device == "cuda":
-        plan.run()
-        th.cuda.synchronize()
-    else:
-        EnsembleInterp(plan).run()
-    return lambda b, shape=None: plan.view(b, shape).cpu().clone()
-
-
-def cases(gpu, cpu):
-    """pytest params: the production-size cases on the GPU, the reduced ones through the interpreter"""
-    return ([pytest.param("cuda", c, marks=pytest.mark.gpu, id="gpu-" + k) for k, c in gpu.items()]
-            + [pytest.param("cpu", c, id="cpu-" + k) for k, c in cpu.items()])
-
-
-def ulp16(ref):
-    """spacing of fp16 numbers at |ref| (2^-24 in the subnormal range)"""
-    return th.exp2(th.floor(th.log2(ref.abs().clamp(min=2.0 ** -14))) - 10)
-
-
-def check(what, got, ref, tol):
-    got, ref = got.to(D64), ref.to(D64)
-    err = (got - ref).abs()
-    bad = ~(err <= tol)  # NaN fails too
-    if bool(bad.any()):
-        j = int(th.nonzero(bad.flatten())[0])
-        tol_j = float(tol.flatten()[j]) if th.is_tensor(tol) and tol.numel() > 1 else float(tol)
-        raise AssertionError(f"{what}: {int(bad.sum())} of {bad.numel()} elements outside tolerance; first at flat index {j}: "
-                             f"got {float(got.flatten()[j])!r}, float64 {float(ref.flatten()[j])!r}, tol {tol_j!r}")
-
-
-def check16(what, got, ref, floor):
-    """fp16 output: one fp16 ulp of the float64 value plus `floor`"""
-    check(what, got, ref, ulp16(ref) + floor)
+from tests.kernel_check import D64, U, cases, check, check16, run, ulp16  # noqa: F401
 
 
 def fp16_values(t):
