@@ -78,8 +78,8 @@ def check(rc: int, what: str = ""):
 
 
 def run_op(code: str, *, flags=0, i=(), f=(), p=(), what=None):
-    """one op outside a plan, on the current CUDA stream: `i` ints, `f` floats, `p` tensors (their data pointers); raises CgdError
-    (prefixed `what`, default the op name) when the library refuses it"""
+    """one op outside a plan, on the current CUDA stream: `i` ints, `f` floats, `p` tensors (their data pointers; None = a null
+    pointer); raises CgdError (prefixed `what`, default the op name) when the library refuses it"""
     import torch as th
     op = CgdOp()
     op.code, op.flags = OP[code], flags
@@ -88,5 +88,5 @@ def run_op(code: str, *, flags=0, i=(), f=(), p=(), what=None):
     for j, v in enumerate(f):
         op.f[j] = float(v)
     for j, t in enumerate(p):
-        op.p[j] = t.data_ptr()
+        op.p[j] = None if t is None else t.data_ptr()
     check(load().cgd_run_op(ctypes.byref(op), ctypes.c_void_p(th.cuda.current_stream().cuda_stream)), what or code.lower())

@@ -5,8 +5,6 @@ residual and QuickGELU' (CONV flags 4) at every BN >= 64, outputs and residuals 
 offset), guard channels around the output slice that must keep their sentinel, multi-image tiles clipped in N, a partial last
 column box, column tiles wholly beyond Cout, BN 32 / 16 (narrower boxes and swizzles), fewer tiles than SMs, and more than 8
 rounds of tiles per CTA."""
-import ctypes
-
 import pytest
 import torch as th
 import torch.nn.functional as F
@@ -51,15 +49,9 @@ NPAD = {"col_tiles_beyond_cout": 256}  # padded weight rows when not the next mu
 
 
 def _conv_op(x, wp, bias, res, out, NB, H, W, Cin, Cout, npad, taps, bn, flags):
-    op = _lib.CgdOp()
-    op.code, op.flags = _lib.OP["CONV"], flags
     rs = res.stride()[:3] if res is not None else (0, 0, 0)
-    i = [NB, H, W, Cin, Cout, npad, taps, *x.stride()[:3], *out.stride()[:3], *rs, bn, 1, 0, 1, 0, 0, 0, 0]
-    for j, v in enumerate(i):
-        op.i[j] = int(v)
-    for j, t in enumerate((x, wp, bias, res, out)):
-        op.p[j] = t.data_ptr() if t is not None else None
-    _lib.check(_lib.load().cgd_run_op(ctypes.byref(op), ctypes.c_void_p(th.cuda.current_stream().cuda_stream)), "conv")
+    _lib.run_op("CONV", flags=flags, i=[NB, H, W, Cin, Cout, npad, taps, *x.stride()[:3], *out.stride()[:3], *rs, bn, 1, 0, 1, 0, 0, 0, 0],
+                p=[x, wp, bias, res, out], what="conv")
 
 
 def _qgelu_grad(u):
