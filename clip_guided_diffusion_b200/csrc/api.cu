@@ -90,6 +90,9 @@ static int dispatch(const CgdOp& op, const ConvTcLaunch* conv, cudaStream_t st) 
     case CGD_OP_FINAL_GRAD: return launch_final_grad(op, st);
     case CGD_OP_SAMPLE_ANCESTRAL: return launch_sample_ancestral(op, st);
     case CGD_OP_SAMPLE_DDIM: return launch_sample_ddim(op, st);
+    case CGD_OP_GRAD_SEED: return launch_grad_seed(op, st);
+    case CGD_OP_GRAD_UNSCALE: return launch_grad_unscale(op, st);
+    case CGD_OP_PMV_BWD: return launch_pmv_bwd(op, st);
     default: set_error("unknown op code %d", op.code); return -1;
   }
 }
@@ -99,6 +102,7 @@ static int op_launches(const CgdOp& op, const ConvTcLaunch* conv) {
     case CGD_OP_CONV: return conv_tc_num_launches(*conv);
     case CGD_OP_ATTN_BWD: return attn_bwd_num_launches(op);
     case CGD_OP_FINAL_GRAD: return ((op.flags & 1) && !(op.flags & 4)) ? 2 : 1;
+    case CGD_OP_GRAD_SEED: return 2;
     default: return 1;
   }
 }

@@ -55,4 +55,7 @@ int launch_guide_grad(const CgdOp& op, cudaStream_t st);
 int launch_final_grad(const CgdOp& op, cudaStream_t st);
 int launch_sample_ancestral(const CgdOp& op, cudaStream_t st);
 int launch_sample_ddim(const CgdOp& op, cudaStream_t st);
+int launch_grad_seed(const CgdOp& op, cudaStream_t st);
+int launch_grad_unscale(const CgdOp& op, cudaStream_t st);
+int launch_pmv_bwd(const CgdOp& op, cudaStream_t st);
 }  // namespace cgd

@@ -9,6 +9,7 @@ kept (they are part of the surface); all per-pixel algebra runs in the CUDA kern
 """
 from __future__ import annotations
 
+import contextlib
 import math
 
 import numpy as np
@@ -114,15 +115,26 @@ class GaussianDiffusion:
         _require(not clip_denoised and denoised_fn is None,
                  "the H100 step implements the reference's configuration (clip_denoised=False, no denoised_fn; cgd/cgd.py:253)")
         engine = _engine_of(model)
-        return engine.unet_forward(self, x, _uniform_t(t), (model_kwargs or {}).get("y"))
+        y = (model_kwargs or {}).get("y")
+        if th.is_grad_enabled() and x.requires_grad:  # the outputs carry a grad_fn back to x through the UNet (input_grad engines)
+            return engine.p_mean_variance_autograd(self, x, _uniform_t(t), y)
+        return engine.unet_forward(self, x, _uniform_t(t), y)
 
     def _step(self, mode, model, x, t, clip_denoised, denoised_fn, cond_fn, model_kwargs, eta=0.0, noise=None):
         engine = _engine_of(model)
         ti = _uniform_t(t)
-        out = self.p_mean_variance(model, x, t, clip_denoised, denoised_fn, model_kwargs)
-        if mode == "ancestral" and noise is None:
-            noise = engine.draw_noise()  # drawn BEFORE cond_fn (SURVEY 3.2)
-        g = cond_fn(x, t, out, **(model_kwargs or {})) if cond_fn is not None else None
+        # on an input_grad engine any cond_fn but the engine's own CondFnB200 gets x with requires_grad=True inside enable_grad, like the
+        # fork's *_with_grad steps, and takes its gradient with th.autograd.grad through p_mean_variance and the UNet
+        generic = cond_fn is not None and getattr(engine, "input_grad", False) and not engine.drives(cond_fn)
+        with th.enable_grad() if generic else contextlib.nullcontext():
+            if generic:
+                x = x.detach().requires_grad_()
+            out = self.p_mean_variance(model, x, t, clip_denoised, denoised_fn, model_kwargs)
+            if mode == "ancestral" and noise is None:
+                noise = engine.draw_noise()  # drawn BEFORE cond_fn (SURVEY 3.2)
+            g = cond_fn(x, t, out, **(model_kwargs or {})) if cond_fn is not None else None
+        if generic:
+            g, out = g.detach(), {k: v.detach() if isinstance(v, th.Tensor) else v for k, v in out.items()}
         if mode == "ddim" and noise is None:
             noise = engine.draw_noise()  # drawn AFTER cond_fn, consumed even when eta == 0 (SURVEY 3.3)
         sample = engine.update(self, mode, ti, g, noise, eta)

@@ -98,7 +98,14 @@ class EngineModel:
         self.dtype = th.float16
 
     def __call__(self, x, timesteps, y=None):
-        return self.engine.unet(x, timesteps, y)
+        """with grad mode on and ``x.requires_grad`` (an input gradient is wanted: a PyTorch cond_fn's ``th.autograd.grad(loss, x)``)
+        the result is a fresh tensor with a ``grad_fn`` whose backward runs the UNet input-gradient plan; otherwise a view of the
+        engine's output buffer, valid until the next UNet forward"""
+        eng = self.engine
+        if th.is_grad_enabled() and isinstance(x, th.Tensor) and x.requires_grad:
+            return _UNetFunction.apply(x, eng, timesteps, y)
+        eng.forward_generation += 1
+        return eng.unet(x, timesteps, y)
 
     def parameters(self):
         yield self.engine.plan.arena
@@ -138,12 +145,44 @@ class EngineModel:
         for flag in ("grid_gn", "fused_gn", "cluster_splitk"):
             setattr(shadow, flag, getattr(eng.plan, flag))
         UNetB200(eng.unet.cfg, state_dict, batch=eng.B, height=eng.H, width=eng.W, device="cpu", seed_scale=eng.unet.seed_scale, plan=shadow,
-                 build_backward=bool(eng.towers))
+                 build_backward=bool(eng.towers) or eng.input_grad)
         eng.plan.reload_consts(shadow, first=0)  # the UNet is the first network of the engine's plan
         if eng.device.type == "cuda":
             th.cuda.synchronize(eng.device)
         import collections
         return collections.namedtuple("IncompatibleKeys", "missing_keys unexpected_keys")(missing, unexpected)
+
+
+class _UNetFunction(th.autograd.Function):
+    """``model(x, t, y)`` under autograd: forward = the UNet forward range; backward = GRAD_SEED -> UNet input-gradient plan ->
+    GRAD_UNSCALE.  The backward re-enters the activations of the engine's arena, so it must follow the latest UNet forward."""
+
+    @staticmethod
+    def forward(ctx, x, eng, timesteps, y):
+        ctx.eng, ctx.gen = eng, eng.autograd_forward(x, timesteps, y)
+        return eng.unet.out_view.clone()
+
+    @staticmethod
+    def backward(ctx, d_out):
+        return ctx.eng.autograd_backward(ctx.gen, d_out=d_out), None, None, None
+
+
+class _PMVFunction(th.autograd.Function):
+    """the package's ``p_mean_variance`` under autograd: forward = UNet forward + PMV_BLEND; backward = PMV_BWD -> GRAD_SEED -> UNet
+    input-gradient plan -> GRAD_UNSCALE (+ the direct x terms of pred_xstart and mean)"""
+
+    @staticmethod
+    def forward(ctx, x, eng, diffusion, t_index, y):
+        out = eng.unet_forward(diffusion, x.detach(), t_index, y)
+        ctx.eng, ctx.gen = eng, eng.forward_generation
+        return tuple(out[k].clone() for k in PMV_KEYS)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        return ctx.eng.autograd_backward(ctx.gen, pmv_grads=grads), None, None, None, None
+
+
+PMV_KEYS = ("pred_xstart", "mean", "variance", "log_variance")
 
 
 def _as_list(v):
@@ -198,8 +237,12 @@ class GuidedStepB200:
                  tv_scale=150.0, range_scale=50.0, sat_scale=0.0, use_magnitude=False, device="cuda", seed_scale=0.0,
                  vit_grad_scale=1.0, conv_impl=0, rank: int = 0, world_size: int = 1, use_graph: bool = True, vit_streams: int = 1,
                  cutn_variants: tuple = (), lpips_sd: dict = None, init_scale: float = 0.0, cutout_resize: str = "pool",
-                 use_augs: bool = False):
+                 use_augs: bool = False, input_grad: bool = False):
+        """``input_grad``: also build the input-gradient path of ``model()`` and of ``p_mean_variance`` under torch.autograd (the UNet
+        backward even without a CLIP tower, and the GRAD_SEED / GRAD_UNSCALE / PMV_BWD ranges after the step's), so any PyTorch cond_fn
+        can guide a run"""
         self.device = th.device(device)
+        self.input_grad = bool(input_grad)
         self.B = batch
         self.rank, self.world = rank, world_size
         self.global_batch = batch * world_size
@@ -221,7 +264,7 @@ class GuidedStepB200:
         self.plan = p = Plan(conv_impl=conv_impl)
         B, H, W, HW = self.B, self.H, self.W, self.H * self.W
         self.unet = UNetB200(unet_cfg, unet_sd, batch=B, height=H, width=W, device=device, seed_scale=seed_scale or 1.0, plan=p,
-                             build_backward=bool(cfgs))
+                             build_backward=bool(cfgs) or self.input_grad)
         n3 = B * 3 * HW
         self.sc = p.new(SC["COUNT"], "f", "scalars")
         self.noise = p.new(n3, "f", "noise")
@@ -329,6 +372,8 @@ class GuidedStepB200:
         p.mark("upd_ddim")
         p.emit("SAMPLE_DDIM", i=[n], p=[(self.unet.x_in, 0), (self.x0, 0), None, (self.noise, 0), (self.sc, 0), (self.sample, 0)])
         p.mark("engine_end")
+        if self.input_grad:  # after engine_end and after every other buffer: the step's ops and offsets stay what they are without it
+            self._emit_input_grad()
         p.finalize(device)
         self.model = EngineModel(self)
         self.shape = (B, 3, H, W)
@@ -351,8 +396,35 @@ class GuidedStepB200:
                                                                                     default=1) - 1)] if self.device.type == "cuda" else []
         self._last_out = None
         self._fwd_valid = False
+        # bumped by every UNet forward (fused step, unet_forward, model()): an autograd backward or an update whose forward is no longer
+        # the latest would differentiate or read someone else's activations
+        self.forward_generation = 0
+        self._pmv_generation = None
         self.h2d_bytes = 0
         self.d2h_bytes = 0
+
+    def _emit_input_grad(self):
+        """the ops of the autograd bridge, each in its own range: PMV_BWD (ag_pmv_bwd), GRAD_SEED (ag_seed), GRAD_UNSCALE without
+        (ag_unscale) and with the direct x term (ag_unscale_d)"""
+        p, B, HW = self.plan, self.B, self.H * self.W
+        n3 = B * 3 * HW
+        self.ag_d_out = p.new(B * 6 * HW, "f", "ag_d_model_out")
+        self.ag_dyn = p.new(2 * B, "f", "ag_seed_dyn")
+        self.ag_dx = p.new(n3, "f", "ag_dx")
+        self.ag_dx_direct = p.new(n3, "f", "ag_dx_direct")
+        self.ag_pmv_grads = p.new(4 * n3, "f", "ag_pmv_grads")  # upstream grads of pred_xstart | mean | variance | log_variance
+        p.mark("ag_pmv_bwd")
+        p.emit("PMV_BWD", i=[B, HW], p=[(self.sc, 0), (self.var, 0)] + [(self.ag_pmv_grads, k * n3) for k in range(4)]
+               + [(self.ag_d_out, 0), (self.ag_dx_direct, 0)], tag="d p_mean_variance")
+        p.mark("ag_seed")
+        p.emit("GRAD_SEED", i=[B, HW, IN_PAD], p=[(self.ag_d_out, 0), (self.ag_dyn, 0), (self.unet.seed, 0)], tag="seed of model() backward")
+        p.mark("ag_unscale")
+        p.emit("GRAD_UNSCALE", i=[B, HW, IN_PAD], p=[(self.unet.dx, 0), None, (self.ag_dyn, 0), (self.unet.seed, 0), (self.ag_dx, 0)],
+               tag="dx of model()")
+        p.mark("ag_unscale_d")
+        p.emit("GRAD_UNSCALE", i=[B, HW, IN_PAD], p=[(self.unet.dx, 0), (self.ag_dx_direct, 0), (self.ag_dyn, 0), (self.unet.seed, 0), (self.ag_dx, 0)],
+               tag="dx of p_mean_variance")
+        p.mark("ag_end")
 
     def _emit_cutouts(self, tw, c, accumulate):
         """cutouts -> CLIP (the tower's own op ranges) -> spherical loss -> cutout gradient into g_clip, for `c` windows of tower `tw`;
@@ -477,6 +549,7 @@ class GuidedStepB200:
     def _run_all(self, mode, runner=None, cutn=None):
         """one guided step launched range by range, without a CUDA graph; ``runner(mark_a, mark_b)`` stands in for
         ``plan.run_range`` (the tests interpret op lists with it)"""
+        self.forward_generation += 1
         self._launch(self.schedule(mode, cutn), runner)
 
     def _launch(self, steps, runner=None):
@@ -504,6 +577,52 @@ class GuidedStepB200:
         ranges = [r for e in self.schedule(mode) if e != ALL_REDUCE for r in (e if isinstance(e, _Fork) else [e])]
         return sum(self.plan.num_launches(m[a], m[b] - m[a]) for a, b in ranges)
 
+    # ------------------------------------------------------------------ torch.autograd bridge (input_grad=True)
+    def _check_autograd_input(self, x):
+        if not self.input_grad:
+            raise RuntimeError("input gradients through the engine's UNet need an engine built with GuidedStepB200(..., input_grad=True)")
+        if tuple(x.shape) != self.shape:
+            raise ValueError(f"engine built for inputs of shape {self.shape}, got {tuple(x.shape)}")
+
+    def autograd_forward(self, x, timesteps, y=None) -> int:
+        """the UNet forward of ``model()`` under autograd; returns its forward generation"""
+        self._check_autograd_input(x)
+        self.unet.set_inputs(x.detach(), timesteps, y)
+        self.forward_generation += 1
+        self.plan.run_range("unet_emb", "unet_bwd")
+        return self.forward_generation
+
+    def p_mean_variance_autograd(self, diffusion, x, t_index, y=None) -> dict:
+        """p_mean_variance whose outputs carry a ``grad_fn`` back to ``x`` (through the UNet and the p_mean_variance algebra)"""
+        self._check_autograd_input(x)
+        out = dict(zip(PMV_KEYS, _PMVFunction.apply(x, self, diffusion, t_index, y)))
+        out["engine"] = self
+        return out
+
+    def autograd_backward(self, generation, d_out=None, pmv_grads=None) -> th.Tensor:
+        """d loss / d x from d loss / d model_out (``d_out``) or from the upstream grads of p_mean_variance's four outputs"""
+        if th.is_grad_enabled():
+            raise RuntimeError("double backward (create_graph=True) through the engine's UNet is not supported")
+        if generation != self.forward_generation:
+            raise RuntimeError("backward through the engine's UNet after another UNet forward ran on this engine: its activations are "
+                               "overwritten (run the backward of each forward before the next forward)")
+        run = self.plan.run_range
+        if pmv_grads is not None:
+            g = self.v(self.ag_pmv_grads, (4,) + self.shape)
+            for k, gk in enumerate(pmv_grads):
+                g[k].copy_(gk) if gk is not None else g[k].zero_()
+            run("ag_pmv_bwd", "ag_seed")
+        else:
+            self.v(self.ag_d_out, (self.B, 6, self.H, self.W)).copy_(d_out)
+        run("ag_seed", "ag_unscale")
+        run("unet_bwd", "unet_end")
+        run(*(("ag_unscale_d", "ag_end") if pmv_grads is not None else ("ag_unscale", "ag_unscale_d")))
+        return self.img(self.ag_dx).clone()
+
+    def drives(self, cond_fn) -> bool:
+        """True for this engine's own CondFnB200: the loops then take the fused / segment guidance kernels instead of autograd"""
+        return isinstance(cond_fn, CondFnB200) and cond_fn.engine is self
+
     # ------------------------------------------------------------------ segment-wise execution (API-parity path)
     def _push_scalars(self, sc: np.ndarray):
         self.v(self.sc).copy_(th.from_numpy(sc), non_blocking=True)
@@ -515,6 +634,8 @@ class GuidedStepB200:
         self._push_scalars(diffusion.scalar_table(t_index, fac_index))
         ts = th.full((self.B,), diffusion.model_timestep(t_index), dtype=th.float32)
         self.unet.set_inputs(x, ts.to(self.device, non_blocking=True), y)
+        self.forward_generation += 1
+        self._pmv_generation = self.forward_generation
         self._launch(self.schedule("ddim", guided=False)[:2])  # UNet forward, p_mean_variance
         self._fwd_valid = True
         out = {"mean": self.img(self.mean), "variance": self.img(self.var), "log_variance": self.img(self.logvar),
@@ -540,6 +661,9 @@ class GuidedStepB200:
         return self.img(self.g)
 
     def update(self, diffusion, mode, t_index, g, noise, eta=0.0) -> th.Tensor:
+        if self._pmv_generation is not None and self._pmv_generation != self.forward_generation:
+            raise RuntimeError("update after another UNet forward ran on this engine: the step's p_mean_variance buffers and x are "
+                               "overwritten (a cond_fn must not call the engine's model itself)")
         if mode == "ddim" and eta != 0.0:
             self.v(self.sc)[SC["ETA"]] = float(eta)
         if noise.data_ptr() != self.v(self.noise).data_ptr():
@@ -686,6 +810,7 @@ class GuidedStepB200:
         """one step from CUDA graphs: the schedule cut at its host all-reduce into segments, one graph per segment, captured on first
         use after one eager run (which sets kernel attributes and touches every buffer), then replayed with the all-reduce between"""
         steps = self.schedule(mode, cutn, guided)
+        self.forward_generation += 1
         if not self.use_graph:
             self._launch(steps)
             return

@@ -242,6 +242,21 @@ enum {
    * p0 x(h [n_src rows, row stride i2]) p1 idx(i32 [rows], 4-byte aligned) p2 y(h [rows, row stride i3]) ; i0 rows i1 w (% 8 == 0) i2 ldx i3 ldy
    * i4 n_src.  An index outside [0, n_src) gives a row of NaNs. */
   CGD_OP_ROW_GATHER = 54,
+  /* The UNet under torch.autograd (clip_guided_diffusion_b200/guidance.py, EngineModel): a cond_fn's d loss / d model_out seeds the
+   * input-gradient plan.  d_out(f NCHW [B,6,HW]) -> seed(h pixel-major [B,HW,ld], channels 0..5) * scale_b, with SEED_QUANT's per-image
+   * power of two: pass 1 puts max_b |d_out| into dyn[b] (atomicMax on the float bits; a NaN is dropped, an inf counts as 3e38; dyn[0..B)
+   * must be 0 on entry), pass 2 scale_b = 2^clamp(floor(log2(4096 / max_b)), -60, 60) (1 for an all-zero image), values saturated at
+   * +-60000, dyn[B + b] = scale_b.  Two launches.  p0 d_out p1 dyn(f [2B]) p2 seed ; i0 B i1 HW i2 ld (even, >= 6) */
+  CGD_OP_GRAD_SEED = 55,
+  /* dx = dx_unet / scale_b (+ dx_direct), then dyn[0..B) = 0 and seed channels 0..5 = 0 (the fused step's GUIDE_GRAD / SEED_QUANT write
+   * channels 0..2 only).  p0 dx_unet(f NCHW [B,3,HW]) p1 dx_direct(f NCHW)|0 p2 dyn(f [2B]) p3 seed(h [B,HW,ld]) p4 dx(f NCHW)
+   * i0 B i1 HW i2 ld */
+  CGD_OP_GRAD_UNSCALE = 56,
+  /* transpose of CGD_OP_PMV_BLEND's p_mean_variance algebra (without the x_in blend): G = g_x0 + c1 g_mean ; d_out[:, 0:3] = -bb G ;
+   * d_out[:, 3:6] = (maxl - minl) / 2 * (g_logvar + variance * g_variance) ; dx_direct = a G + c2 g_mean.
+   * p0 sc p1 variance(f NCHW [B,3,HW], needed with p4) p2 g_pred_xstart|0 p3 g_mean|0 p4 g_variance|0 p5 g_log_variance|0
+   * p6 d_out(f NCHW [B,6,HW]) p7 dx_direct(f NCHW [B,3,HW]) ; i0 B i1 HW */
+  CGD_OP_PMV_BWD = 57,
   CGD_OP__COUNT
 };
 
