@@ -93,6 +93,9 @@ static int dispatch(const CgdOp& op, const ConvTcLaunch* conv, cudaStream_t st) 
     case CGD_OP_GRAD_SEED: return launch_grad_seed(op, st);
     case CGD_OP_GRAD_UNSCALE: return launch_grad_unscale(op, st);
     case CGD_OP_PMV_BWD: return launch_pmv_bwd(op, st);
+    case CGD_OP_CLIP_PATCHIFY: return launch_clip_patchify(op, st);
+    case CGD_OP_CLIP_SEED: return launch_clip_seed(op, st);
+    case CGD_OP_CLIP_UNPATCHIFY: return launch_clip_unpatchify(op, st);
     default: set_error("unknown op code %d", op.code); return -1;
   }
 }

@@ -58,4 +58,7 @@ int launch_sample_ddim(const CgdOp& op, cudaStream_t st);
 int launch_grad_seed(const CgdOp& op, cudaStream_t st);
 int launch_grad_unscale(const CgdOp& op, cudaStream_t st);
 int launch_pmv_bwd(const CgdOp& op, cudaStream_t st);
+int launch_clip_patchify(const CgdOp& op, cudaStream_t st);
+int launch_clip_seed(const CgdOp& op, cudaStream_t st);
+int launch_clip_unpatchify(const CgdOp& op, cudaStream_t st);
 }  // namespace cgd

@@ -257,6 +257,24 @@ enum {
    * p0 sc p1 variance(f NCHW [B,3,HW], needed with p4) p2 g_pred_xstart|0 p3 g_mean|0 p4 g_variance|0 p5 g_log_variance|0
    * p6 d_out(f NCHW [B,6,HW]) p7 dx_direct(f NCHW [B,3,HW]) ; i0 B i1 HW */
   CGD_OP_PMV_BWD = 57,
+  /* A CLIP visual tower under torch.autograd (clip_guided_diffusion_b200/clip_model.py, load_clip): a user's NCHW image batch becomes the
+   * tower's patch rows, k = (c, ky, kx) within a P x P patch, G = R / P patches per side (the ViTs' patch size, P = 2 for the ModifiedResNet
+   * towers' space-to-depth stem).  patches[b, gy*G + gx, c*P*P + ky*P + kx] = fp16_rn(x[b, c, gy*P + ky, gx*P + kx]) for b < n; columns
+   * 3*P*P..kpad and rows n..n_built are zero.  One rounding per element, 128-bit stores.
+   * p0 x(f NCHW [n,3,R,R]) p1 patches(h [n_built, G*G, kpad], 16-byte aligned) ; i0 n i1 n_built i2 R i3 P i4 kpad (% 8 == 0, >= 3*P*P) */
+  CGD_OP_CLIP_PATCHIFY = 58,
+  /* the dynamic loss scale of the tower backward, one CTA per image: m_b = max |d[b, :]| (a NaN is dropped, an inf counts as 3e38),
+   * scale_b = 2^clamp(floor(log2(f0 / m_b)), -60, 60) (1 for an all-zero row), d_embeds[b, :] = d[b, :] * scale_b, dyn[b] = scale_b;
+   * rows n..n_built get zeros and scale 1.  f0 = BAND, the target of the largest seed value: 2^9 (clip_model.py CLIP_SEED_BAND), the
+   * largest power of two that left 2^4 or more of headroom below 65504 in every fp16 gradient buffer of the seeded ViT-B/32, ViT-B/16,
+   * ViT-L/14 and RN50 towers at 16 images: 2^4.46 (ViT-B/16) to 2^6.88 (RN50) on an H100 (scripts/clip_seed_band.py, DESIGN.md section 2;
+   * seeded weights, not the published checkpoints).
+   * p0 d(f [n_built, D]) p1 d_embeds(f [n_built, D]) p2 dyn(f [n_built]) ; i0 n i1 n_built i2 D (<= 1024) ; f0 BAND (a power of two) */
+  CGD_OP_CLIP_SEED = 59,
+  /* transpose of CGD_OP_CLIP_PATCHIFY with the seed's scale undone: dx[b, c, gy*P + ky, gx*P + kx] = float(d_patches[b, gy*G + gx,
+   * c*P*P + ky*P + kx]) * (1 / dyn[b]) for b < n (exact: the scale is a power of two); pad columns and rows n.. are not read.
+   * p0 d_patches(h [n_built, G*G, kpad]) p1 dyn(f [n_built]) p2 dx(f NCHW [n,3,R,R]) ; i0 n i1 n_built i2 R i3 P i4 kpad */
+  CGD_OP_CLIP_UNPATCHIFY = 60,
   CGD_OP__COUNT
 };
 

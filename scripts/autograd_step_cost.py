@@ -6,7 +6,11 @@
 - generic: the same guidance written in PyTorch -- the oracle's cond_fn with the CLIP tower in fp16 (LayerNorm in fp32, like the
   reference's clip.model.convert_weights) -- through the package's ddim_sample_with_grad on an input_grad engine: UNet forward +
   p_mean_variance on the engine, CLIP forward / backward in PyTorch, the UNet input gradient on the engine;
-- unet_fwd_bwd: `model()` forward + `th.autograd.grad` alone, no guidance.
+- unet_fwd_bwd: `model()` forward + `th.autograd.grad` alone, no guidance;
+- generic_engine_clip: the generic step with load_clip's model (clip_model.py) in place of the eager fp16 tower, so both networks run on
+  the engine's kernels (timed alternating with a second run of the generic step);
+- clip_fwd_bwd: `encode_image` + `th.autograd.grad` alone, load_clip's model against the eager fp16 tower, for ViT-B/32, ViT-B/16,
+  ViT-L/14 and RN50 at 16 and 64 images (timed alternating).
 
 CUDA events around each step, warmed up, medians over the timed steps.  Prints one JSON line with the card's name and power limit.
 
@@ -46,6 +50,72 @@ def timed(fn, steps, warmup):
         b.synchronize()
         ms.append(a.elapsed_time(b))
     return statistics.median(ms)
+
+
+def timed_alternating(fns: dict, steps, warmup):
+    """{name: median ms}: every fn warmed up, then the timed calls interleaved (a, b, a, b, ...) so that clock or thermal drift hits
+    all arms alike"""
+    for fn in fns.values():
+        for _ in range(warmup):
+            fn()
+    th.cuda.synchronize()
+    ms = {k: [] for k in fns}
+    for _ in range(steps):
+        for k, fn in fns.items():
+            a, b = th.cuda.Event(enable_timing=True), th.cuda.Event(enable_timing=True)
+            a.record()
+            fn()
+            b.record()
+            b.synchronize()
+            ms[k].append(a.elapsed_time(b))
+    return {k: statistics.median(v) for k, v in ms.items()}
+
+
+def eager_fp16(tower):
+    """the oracle tower the way the reference runs CLIP on CUDA: fp16 weights, normalisation layers in fp32"""
+    tower = tower.cuda().half()
+    for m in tower.modules():
+        if isinstance(m, (th.nn.LayerNorm, th.nn.BatchNorm2d)):
+            m.float()
+    for prm in tower.parameters():
+        prm.requires_grad_(False)
+    return tower
+
+
+def clip_fwd_bwd(steps, warmup):
+    """encode_image + autograd.grad of the input, engine (load_clip) vs eager fp16, per tower and image count"""
+    from clip_guided_diffusion_b200 import clip_util
+    from clip_guided_diffusion_b200 import rn as prn
+    from oracle import clip_rn as orn
+    from oracle.clip_vit import VIT_CONFIGS, CLIPVisualOnly
+    out = {}
+    for name in ("ViT-B/32", "ViT-B/16", "ViT-L/14", "RN50"):
+        if name in pv.VIT_CONFIGS:
+            cfg = pv.VIT_CONFIGS[name]
+            sd = pw.seeded_state_dict(pw.vit_param_shapes(cfg), 1235)
+            eager = CLIPVisualOnly(VIT_CONFIGS[name]).eval()
+            eager.load_state_dict(sd)
+        else:
+            cfg = prn.RN_CONFIGS[name]
+            sd = pw.seeded_rn_state_dict(cfg, seed=3)
+            eager = orn.CLIPVisualRN(orn.RNConfig(tuple(cfg.layers), cfg.output_dim, cfg.input_resolution, cfg.width)).eval()
+            eager.load_state_dict(sd, strict=False)
+        eager = eager_fp16(eager)
+        R, D = cfg.input_resolution, cfg.output_dim
+        for n in (16, 64):
+            model, _ = clip_util.load_clip(name, "cuda", clip_state_dict=sd, max_images=n)
+            x = th.randn(n, 3, R, R, device="cuda")
+            w = th.randn(n, D, device="cuda")
+
+            def run(m):
+                def fn():
+                    xe = x.detach().requires_grad_()
+                    return th.autograd.grad((w * m.encode_image(xe).float()).sum(), xe)
+                return fn
+            out[f"{name} x{n}"] = timed_alternating({"engine": run(model), "eager_fp16": run(eager)}, steps, warmup)
+            del model
+            th.cuda.empty_cache()
+    return out
 
 
 def card():
@@ -100,6 +170,17 @@ def main():
         xe = x.detach().requires_grad_()
         return th.autograd.grad((w * geng.model(xe, ts, y)).sum(), xe)
     res["unet_fwd_bwd_ms"] = timed(unet_fwd_bwd, args.steps, args.warmup)
+
+    from clip_guided_diffusion_b200 import clip_util
+    eclip, _ = clip_util.load_clip("ViT-B/32", "cuda", clip_state_dict=vsd, max_images=16)
+    econd = og.OracleCondFn(diff, eclip, tgt.cuda(), th.ones(1, device="cuda"), cut_size=224, num_cutouts=16)
+    econd.current_timestep = 30
+    pair = timed_alternating({c: (lambda c=c: diff.ddim_sample_with_grad(geng.model, x, t, clip_denoised=False, cond_fn=c, model_kwargs={"y": y}))
+                              for c in (ocond, econd)}, args.steps, args.warmup)
+    res["generic_step_ms_alternating"], res["generic_engine_clip_step_ms"] = pair[ocond], pair[econd]
+    del geng, eclip
+    th.cuda.empty_cache()
+    res["clip_fwd_bwd_ms"] = clip_fwd_bwd(args.steps, args.warmup)
     print(json.dumps(res))
 
 
