@@ -24,7 +24,7 @@ OP = dict(CONV=1, GN_STATS=2, GN_APPLY=3, GN_BWD_STATS=4, GN_BWD_APPLY=5, POOL2=
           GN_FWD_FUSED=33, GN_BWD_FUSED=34, GN_FWD_GRID=35, GN_BWD_GRID=36,
           RELU_FWD=37, RELU_BWD=38, MAXPOOL2_FWD=39, MAXPOOL2_BWD=40, LPIPS_TAP=41, FILL=42, CUTOUTS_RR_FWD=43, CUTOUTS_RR_BWD=44, SEED_QUANT=45, MAG_CLAMP=46, ATTNPOOL_EMBED_FWD=47, ATTNPOOL_EMBED_BWD=48, CUTOUTS_AUG_FWD=50, CUTOUTS_AUG_BWD=51,
           RESIZE_AXIS=52, TOKEN_EMBED=53, ROW_GATHER=54, GRAD_SEED=55, GRAD_UNSCALE=56, PMV_BWD=57,
-          CLIP_PATCHIFY=58, CLIP_SEED=59, CLIP_UNPATCHIFY=60)
+          CLIP_PATCHIFY=58, CLIP_SEED=59, CLIP_UNPATCHIFY=60, LPIPS_PAIR_FWD=61, LPIPS_LOSS=62, LPIPS_SEED=63, LPIPS_PAIR_BWD=64)
 SC = dict(SQRT_RECIP_AC=0, SQRT_RECIPM1_AC=1, POST_COEF1=2, POST_COEF2=3, MIN_LOG=4, MAX_LOG=5, FAC=6, NONZERO=7,
           SQRT_1M_AC=8, AC_PREV=9, AC=10, ETA=11, ONE_MINUS_FAC=12, COUNT=16)
 

@@ -96,6 +96,10 @@ static int dispatch(const CgdOp& op, const ConvTcLaunch* conv, cudaStream_t st) 
     case CGD_OP_CLIP_PATCHIFY: return launch_clip_patchify(op, st);
     case CGD_OP_CLIP_SEED: return launch_clip_seed(op, st);
     case CGD_OP_CLIP_UNPATCHIFY: return launch_clip_unpatchify(op, st);
+    case CGD_OP_LPIPS_PAIR_FWD: return launch_lpips_pair_fwd(op, st);
+    case CGD_OP_LPIPS_LOSS: return launch_lpips_loss(op, st);
+    case CGD_OP_LPIPS_SEED: return launch_lpips_seed(op, st);
+    case CGD_OP_LPIPS_PAIR_BWD: return launch_lpips_pair_bwd(op, st);
     default: set_error("unknown op code %d", op.code); return -1;
   }
 }

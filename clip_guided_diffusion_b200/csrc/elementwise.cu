@@ -175,7 +175,7 @@ __global__ void nchw_to_pm_kernel(const float* __restrict__ src, __half* __restr
 // pixel-major (fp16 / fp32) -> fp32 NCHW, one thread per destination element (reads of a pixel's few channels hit one sector)
 template <typename T>
 __global__ void pm_to_nchw_kernel(const T* __restrict__ src, float* __restrict__ dst, int N, int C, int64_t HW, int64_t ld, float scale,
-                                  int accumulate, float3 mul) {
+                                  int accumulate, float3 mul, const float* __restrict__ div) {
   pdl_wait();
   pdl_launch_dependents();
   const int64_t total = (int64_t)N * C * HW;
@@ -184,7 +184,8 @@ __global__ void pm_to_nchw_kernel(const T* __restrict__ src, float* __restrict__
     const int64_t nc = idx / HW;
     const int c = (int)(nc % C);
     const int64_t n = nc / C;
-    const float v = (float)src[(n * HW + p) * ld + c] * scale * (c == 0 ? mul.x : (c == 1 ? mul.y : mul.z));
+    float v = (float)src[(n * HW + p) * ld + c] * scale * (c == 0 ? mul.x : (c == 1 ? mul.y : mul.z));
+    if (div) v = v / div[n];
     dst[idx] = accumulate ? dst[idx] + v : v;
   }
 }
@@ -205,10 +206,13 @@ int launch_pm_to_nchw(const CgdOp& op, cudaStream_t st) {
   const int acc = (op.flags & 2) ? 1 : 0;
   CGD_CHECK_ARG(!(op.flags & 4) || C <= 3, "pm_to_nchw: per-channel scale needs C <= 3");
   const float3 mul = (op.flags & 4) ? make_float3(op.f[1], op.f[2], op.f[3]) : make_float3(1.f, 1.f, 1.f);  // per-channel multiplier
+  // flags 8: image n divided by div[n] (p2, fp32 [N]; the per-image power-of-two scale of a seeded backward)
+  CGD_CHECK_ARG(!(op.flags & 8) || (op.p[2] && ((uintptr_t)op.p[2] & 3) == 0), "pm_to_nchw: flags 8 needs a 4-byte aligned divisor vector p2");
+  const float* div = (op.flags & 8) ? (const float*)op.p[2] : nullptr;
   if (op.flags & 1)
-    CGD_CUDA(launch_pdl(pm_to_nchw_kernel<float>, dim3(ew_blocks(N * C * HW)), dim3(256), 0, st, (const float*)op.p[0], (float*)op.p[1], (int)N, (int)C, HW, ld, op.f[0], acc, mul));
+    CGD_CUDA(launch_pdl(pm_to_nchw_kernel<float>, dim3(ew_blocks(N * C * HW)), dim3(256), 0, st, (const float*)op.p[0], (float*)op.p[1], (int)N, (int)C, HW, ld, op.f[0], acc, mul, div));
   else
-    CGD_CUDA(launch_pdl(pm_to_nchw_kernel<__half>, dim3(ew_blocks(N * C * HW)), dim3(256), 0, st, (const __half*)op.p[0], (float*)op.p[1], (int)N, (int)C, HW, ld, op.f[0], acc, mul));
+    CGD_CUDA(launch_pdl(pm_to_nchw_kernel<__half>, dim3(ew_blocks(N * C * HW)), dim3(256), 0, st, (const __half*)op.p[0], (float*)op.p[1], (int)N, (int)C, HW, ld, op.f[0], acc, mul, div));
   CGD_LAUNCH_CHECK();
   return 0;
 }

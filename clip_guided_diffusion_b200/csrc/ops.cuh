@@ -61,4 +61,8 @@ int launch_pmv_bwd(const CgdOp& op, cudaStream_t st);
 int launch_clip_patchify(const CgdOp& op, cudaStream_t st);
 int launch_clip_seed(const CgdOp& op, cudaStream_t st);
 int launch_clip_unpatchify(const CgdOp& op, cudaStream_t st);
+int launch_lpips_pair_fwd(const CgdOp& op, cudaStream_t st);
+int launch_lpips_loss(const CgdOp& op, cudaStream_t st);
+int launch_lpips_seed(const CgdOp& op, cudaStream_t st);
+int launch_lpips_pair_bwd(const CgdOp& op, cudaStream_t st);
 }  // namespace cgd

@@ -114,7 +114,8 @@ enum {
    * flags 4 (C <= 3): per-channel affine (x - f[1+c]) * f[4+c] * f0 (the LPIPS ScalingLayer) */
   CGD_OP_NCHW_TO_PM = 14,
   /* pixel-major (h, or f with flag 1) -> fp32 NCHW (first C channels): p0 src p1 dst ; i0 N i1 C i2 HW i3 ld ; f0 scale
-   * flags 1 = src fp32, 2 = accumulate, 4 (C <= 3) = per-channel multiplier f[1+c] */
+   * flags 1 = src fp32, 2 = accumulate, 4 (C <= 3) = per-channel multiplier f[1+c], 8 = image n divided by p2[n] (fp32 [N]: the
+   * per-image power-of-two scale of LPIPS_SEED, so the division is exact) */
   CGD_OP_PM_TO_NCHW = 15,
   /* LayerNorm rows: p0 x(h) p1 gamma(f) p2 beta(f) p3 y(h) p4 stats(f [rows,2]) ; i0 rows i1 w i2 ldx i3 ldy ; f0 eps (SURVEY K15) */
   CGD_OP_LN_FWD = 16,
@@ -275,6 +276,30 @@ enum {
    * c*P*P + ky*P + kx]) * (1 / dyn[b]) for b < n (exact: the scale is a power of two); pad columns and rows n.. are not read.
    * p0 d_patches(h [n_built, G*G, kpad]) p1 dyn(f [n_built]) p2 dx(f NCHW [n,3,R,R]) ; i0 n i1 n_built i2 R i3 P i4 kpad */
   CGD_OP_CLIP_UNPATCHIFY = 60,
+  /* LPIPS(in0, in1) under torch.autograd (clip_guided_diffusion_b200/lpips.py, LPIPS): one VGG16 trunk per side over the same weights,
+   * tap features f0 (h [N0, HW, C]) and f1 (h [N1, HW, C]) post-ReLU, N0 and N1 each B or 1 (row 0 broadcast over the B images).
+   * Per tap, per pixel: sum_c w_c (f0_c / (||f0|| + 1e-10) - f1_c / (||f1|| + 1e-10))^2.  Nothing normalised is stored, no atomics.
+   * LPIPS_PAIR_FWD: grid (nblk, B) of 8-warp CTAs, each CTA's pixel sum (fixed order) into partial[b * nblk + cta].
+   * p0 f0 p1 f1 p2 w(f [C]) p3 partial(f [B, nblk]) ; i0 B i1 HW i2 C (% 8 == 0, <= 512) i3 N0 i4 N1 i5 nblk (1..4096) */
+  CGD_OP_LPIPS_PAIR_FWD = 61,
+  /* loss[b] = sum over taps k = 0..4 in order of (sum of tap k's nblk_k partials of image b, fixed order) * f_k (= 1 / HW_k): two runs give
+   * the same bits.  p0..p4 partials of taps 0..4 p5 loss(f [B]) ; i0 B i1..i5 nblk of taps 0..4 ; f0..f4 1 / HW of taps 0..4 */
+  CGD_OP_LPIPS_LOSS = 62,
+  /* the dynamic loss scale of the two trunk backwards from the upstream d_loss alone (the backward is linear in it): for trunk row j of
+   * [trunk 0's N0 rows | trunk 1's N1 rows], m = |d_loss[b]| for a row of its own image b, the maximum over all B images for a broadcast
+   * row (a NaN is dropped, an inf counts as 3e38); dyn[j] = 2^clamp(floor(log2(f0 / m)), -60, 60), 1 where m == 0.  f0 = BAND, the
+   * target of |d_loss| * scale: 2^23 (lpips.py LPIPS_SEED_BAND), the largest power of two that left 2^4 or more of headroom below 65504
+   * in every fp16 gradient buffer at 64^2, 256^2 and 512^2 on seeded weights (scripts/lpips_seed_band.py, DESIGN.md section 2).
+   * p0 d_loss(f [B]) p1 dyn(f [N0 + N1]) ; i0 B i1 N0 i2 N1 ; f0 BAND (a power of two in [1, 2^30]) */
+  CGD_OP_LPIPS_SEED = 63,
+  /* the per-tap seeds of the trunk backwards: d f_side[row] = sum over the images b the row serves (in order, fp32) of
+   * (d_loss[b] * dyn[row]) / HW * d LPIPS_tap_b / d f_side[row], rounded once to fp16.  Finite values saturate at +-60000 (like GRAD_SEED);
+   * inf and NaN pass, so a non-finite d_loss[b] gives a non-finite seed and never a finite wrong one.  Deviation from the fp32 math: at a
+   * pixel where every channel of the tap is zero after ReLU the factor 1 / (||f|| + 1e-10) makes the true gradient ~1e10 times its usual
+   * size; the seed holds +-60000 there instead of overflowing to inf (the fused LPIPS_TAP would store inf).
+   * p0 f0 p1 f1 p2 w(f [C]) p3 d_loss(f [B]) p4 dyn(f [N0 + N1]) p5 d f0(h [N0, HW, C])|0 p6 d f1(h [N1, HW, C])|0 ;
+   * i0 B i1 HW i2 C i3 N0 i4 N1 ; flags 1 = write d f0, 2 = write d f1 (p5 / p6 set exactly for the selected sides) */
+  CGD_OP_LPIPS_PAIR_BWD = 64,
   CGD_OP__COUNT
 };
 

@@ -10,7 +10,12 @@
 - generic_engine_clip: the generic step with load_clip's model (clip_model.py) in place of the eager fp16 tower, so both networks run on
   the engine's kernels (timed alternating with a second run of the generic step);
 - clip_fwd_bwd: `encode_image` + `th.autograd.grad` alone, load_clip's model against the eager fp16 tower, for ViT-B/32, ViT-B/16,
-  ViT-L/14 and RN50 at 16 and 64 images (timed alternating).
+  ViT-L/14 and RN50 at 16 and 64 images (timed alternating);
+- lpips_fwd_bwd: `LPIPS()(x_in, init)` + `th.autograd.grad` into x_in alone (init one broadcast image), lpips.py's LPIPS against the eager
+  fp32 oracle.lpips.LPIPSVgg (torch's default cuDNN settings; the same F.conv2d sequence as the `lpips` package), at 256^2 and 512^2,
+  batch 1 and 4 (timed alternating);
+- init_step: the generic step with an init image (init_scale 1000): the oracle's cond_fn on load_clip's model, LPIPS and engine.model,
+  against the fused step of an engine built with the same LPIPS weights (timed alternating).
 
 CUDA events around each step, warmed up, medians over the timed steps.  Prints one JSON line with the card's name and power limit.
 
@@ -118,6 +123,55 @@ def clip_fwd_bwd(steps, warmup):
     return out
 
 
+def lpips_fwd_bwd(steps, warmup):
+    """LPIPS forward + autograd.grad into x_in, lpips.py's LPIPS vs the eager fp32 oracle, per size and batch"""
+    from clip_guided_diffusion_b200 import lpips as pl
+    from oracle import lpips as ol
+    sd = ol.seeded_state_dict()
+    eager = ol.LPIPSVgg({k: v.cuda() for k, v in sd.items()}).cuda()
+    out = {}
+    for size in (256, 512):
+        for n in (1, 4):
+            model = pl.LPIPS(lpips_state_dict=sd)
+            x, init = th.rand(n, 3, size, size, device="cuda") * 2 - 1, th.rand(1, 3, size, size, device="cuda") * 2 - 1
+
+            def run(m):
+                def fn():
+                    xe = x.detach().requires_grad_()
+                    return th.autograd.grad(m(xe, init).sum() * 1000.0, xe)
+                return fn
+            out[f"{size}x{size} x{n}"] = timed_alternating({"engine": run(model), "eager_fp32": run(eager)}, steps, warmup)
+            del model
+            th.cuda.empty_cache()
+    return out
+
+
+def init_step(steps, warmup, ucfg, usd, vcfg, vsd, diff, tgt, x, y):
+    """cfg2 DDIM step with an init image: fused (CondFnB200 with LPIPS) vs generic (OracleCondFn, load_clip, LPIPS, engine.model)"""
+    from clip_guided_diffusion_b200 import clip_util
+    from clip_guided_diffusion_b200 import lpips as pl
+    from oracle import guidance as og
+    from oracle import lpips as ol
+    lsd = ol.seeded_state_dict()
+    init = th.rand(1, 3, 256, 256, device="cuda") * 2 - 1
+    eng = pg.GuidedStepB200(ucfg, usd, vcfg, vsd, batch=1, num_cutouts=16, device="cuda", lpips_sd=lsd, init_scale=1000.0)
+    eng.set_targets(tgt, th.ones(1))
+    eng.set_init_image(init)
+    cond = pg.CondFnB200(eng, diff, pg.MakeCutouts(224, 16))
+    geng = pg.GuidedStepB200(ucfg, usd, batch=1, device="cuda", input_grad=True)
+    eclip, _ = clip_util.load_clip("ViT-B/32", "cuda", clip_state_dict=vsd, max_images=16)
+    ocond = og.OracleCondFn(diff, eclip, tgt.cuda(), th.ones(1, device="cuda"), cut_size=224, num_cutouts=16, lpips_model=pl.LPIPS(lpips_state_dict=lsd),
+                            init_tensor=init, init_scale=1000.0)
+    ocond.current_timestep = 30
+    t = th.full((1,), 30, dtype=th.long, device="cuda")
+    res = timed_alternating({"fused": lambda: eng.fused_step(diff, "ddim", 30, x, y, cond),
+                             "generic": lambda: diff.ddim_sample_with_grad(geng.model, x, t, clip_denoised=False, cond_fn=ocond, model_kwargs={"y": y})},
+                            steps, warmup)
+    del eng, cond, geng, eclip, ocond
+    th.cuda.empty_cache()
+    return res
+
+
 def card():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
     return q.stdout.strip() if q.returncode == 0 else th.cuda.get_device_name(0)
@@ -129,6 +183,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--only", choices=["lpips"], help="only the LPIPS arms (lpips_fwd_bwd, init_step)")
     args = ap.parse_args()
     if not th.cuda.is_available():
         raise SystemExit("needs a GPU: the timings are CUDA events")
@@ -139,6 +194,12 @@ def main():
     tgt = th.randn(1, 512)
     y = th.zeros(1, dtype=th.long, device="cuda")
     res = {"card": card(), "size": "cfg2: 256x256, ViT-B/32, 16 cutouts, batch 1, DDIM", "steps": args.steps, "warmup": args.warmup}
+    if args.only == "lpips":
+        x = th.randn(1, 3, 256, 256, device="cuda")
+        res["init_step_ms"] = init_step(args.steps, args.warmup, ucfg, usd, vcfg, vsd, diff, tgt, x, y)
+        res["lpips_fwd_bwd_ms"] = lpips_fwd_bwd(args.steps, args.warmup)
+        print(json.dumps(res))
+        return
 
     eng = pg.GuidedStepB200(ucfg, usd, vcfg, vsd, batch=1, num_cutouts=16, device="cuda")
     eng.set_targets(tgt, th.ones(1))
@@ -181,6 +242,8 @@ def main():
     del geng, eclip
     th.cuda.empty_cache()
     res["clip_fwd_bwd_ms"] = clip_fwd_bwd(args.steps, args.warmup)
+    res["init_step_ms"] = init_step(args.steps, args.warmup, ucfg, usd, vcfg, vsd, diff, tgt, x, y)
+    res["lpips_fwd_bwd_ms"] = lpips_fwd_bwd(args.steps, args.warmup)
     print(json.dumps(res))
 
 
