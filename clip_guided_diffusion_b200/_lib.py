@@ -24,7 +24,8 @@ OP = dict(CONV=1, GN_STATS=2, GN_APPLY=3, GN_BWD_STATS=4, GN_BWD_APPLY=5, POOL2=
           GN_FWD_FUSED=33, GN_BWD_FUSED=34, GN_FWD_GRID=35, GN_BWD_GRID=36,
           RELU_FWD=37, RELU_BWD=38, MAXPOOL2_FWD=39, MAXPOOL2_BWD=40, LPIPS_TAP=41, FILL=42, CUTOUTS_RR_FWD=43, CUTOUTS_RR_BWD=44, SEED_QUANT=45, MAG_CLAMP=46, ATTNPOOL_EMBED_FWD=47, ATTNPOOL_EMBED_BWD=48, CUTOUTS_AUG_FWD=50, CUTOUTS_AUG_BWD=51,
           RESIZE_AXIS=52, TOKEN_EMBED=53, ROW_GATHER=54, GRAD_SEED=55, GRAD_UNSCALE=56, PMV_BWD=57,
-          CLIP_PATCHIFY=58, CLIP_SEED=59, CLIP_UNPATCHIFY=60, LPIPS_PAIR_FWD=61, LPIPS_LOSS=62, LPIPS_SEED=63, LPIPS_PAIR_BWD=64)
+          CLIP_PATCHIFY=58, CLIP_SEED=59, CLIP_UNPATCHIFY=60, LPIPS_PAIR_FWD=61, LPIPS_LOSS=62, LPIPS_SEED=63, LPIPS_PAIR_BWD=64,
+          IMG_LOSS_FWD=65, IMG_LOSS_BWD=66, SPH_DIST_FWD=67, SPH_DIST_BWD=68)
 SC = dict(SQRT_RECIP_AC=0, SQRT_RECIPM1_AC=1, POST_COEF1=2, POST_COEF2=3, MIN_LOG=4, MAX_LOG=5, FAC=6, NONZERO=7,
           SQRT_1M_AC=8, AC_PREV=9, AC=10, ETA=11, ONE_MINUS_FAC=12, COUNT=16)
 
@@ -80,8 +81,11 @@ def check(rc: int, what: str = ""):
 
 def run_op(code: str, *, flags=0, i=(), f=(), p=(), what=None):
     """one op outside a plan, on the current CUDA stream: `i` ints, `f` floats, `p` tensors (their data pointers; None = a null
-    pointer); raises CgdError (prefixed `what`, default the op name) when the library refuses it"""
+    pointer); raises CgdError (prefixed `what`, default the op name) when an operand is not on a CUDA device or the library refuses it"""
     import torch as th
+    for t in p:
+        if t is not None and not t.is_cuda:
+            raise CgdError(f"{what or code.lower()}: an operand is on {t.device}: the kernels run on the GPU only (no CPU fallback)")
     op = CgdOp()
     op.code, op.flags = OP[code], flags
     for j, v in enumerate(i):

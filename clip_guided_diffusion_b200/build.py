@@ -10,7 +10,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libcgd_b200.so")
-SOURCES = ["api.cu", "conv_tc.cu", "conv_narrow.cu", "norm.cu", "norm_fused.cu", "norm_grid.cu", "norm_grid2.cu", "elementwise.cu", "attention.cu", "attention_small.cu", "attention_flash.cu", "guidance.cu", "augs.cu", "lpips.cu", "linear_small.cu", "resample.cu", "text.cu", "autograd.cu", "clip_autograd.cu"]
+SOURCES = ["api.cu", "conv_tc.cu", "conv_narrow.cu", "norm.cu", "norm_fused.cu", "norm_grid.cu", "norm_grid2.cu", "elementwise.cu", "attention.cu", "attention_small.cu", "attention_flash.cu", "guidance.cu", "augs.cu", "lpips.cu", "linear_small.cu", "resample.cu", "text.cu", "autograd.cu", "clip_autograd.cu", "losses.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "--use_fast_math=false"]
 

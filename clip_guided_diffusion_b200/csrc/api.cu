@@ -100,6 +100,10 @@ static int dispatch(const CgdOp& op, const ConvTcLaunch* conv, cudaStream_t st) 
     case CGD_OP_LPIPS_LOSS: return launch_lpips_loss(op, st);
     case CGD_OP_LPIPS_SEED: return launch_lpips_seed(op, st);
     case CGD_OP_LPIPS_PAIR_BWD: return launch_lpips_pair_bwd(op, st);
+    case CGD_OP_IMG_LOSS_FWD: return launch_img_loss_fwd(op, st);
+    case CGD_OP_IMG_LOSS_BWD: return launch_img_loss_bwd(op, st);
+    case CGD_OP_SPH_DIST_FWD: return launch_sph_dist_fwd(op, st);
+    case CGD_OP_SPH_DIST_BWD: return launch_sph_dist_bwd(op, st);
     default: set_error("unknown op code %d", op.code); return -1;
   }
 }
@@ -110,6 +114,7 @@ static int op_launches(const CgdOp& op, const ConvTcLaunch* conv) {
     case CGD_OP_ATTN_BWD: return attn_bwd_num_launches(op);
     case CGD_OP_FINAL_GRAD: return ((op.flags & 1) && !(op.flags & 4)) ? 2 : 1;
     case CGD_OP_GRAD_SEED: return 2;
+    case CGD_OP_IMG_LOSS_FWD: return 2;
     default: return 1;
   }
 }

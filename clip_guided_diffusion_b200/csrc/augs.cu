@@ -167,8 +167,12 @@ __global__ void cutouts_aug_fwd_kernel(const float* __restrict__ x, const int* _
 }
 
 // ---------------------------------------------------------------- backward: the transposed gather, scattered with fp32 atomics
-// dx must be zero on entry (CGD_OP_FILL before this op); dx += d loss / d x_in of the CLIP path
-__global__ void cutouts_aug_bwd_kernel(const __half* __restrict__ dpatch, const int* __restrict__ coords, const float* __restrict__ params,
+// dx must be zero on entry (CGD_OP_FILL before this op); dx += d loss / d x_in of the CLIP path.  InT = float (flags 4): fp32 d cutouts
+// [cutn*B, 3, cs, cs] of the stand-alone MakeCutouts backward (the patch layout with P = cs, Kpad = 3 cs^2)
+__device__ __forceinline__ float aug_in(const __half* p) { return __half2float(*p); }
+__device__ __forceinline__ float aug_in(const float* p) { return *p; }
+template <typename InT>
+__global__ void cutouts_aug_bwd_kernel(const InT* __restrict__ dpatch, const int* __restrict__ coords, const float* __restrict__ params,
                                        float* __restrict__ dx, int B, int H, int W, int cutn, int cs, int P, int Kpad, float3 stdv, float scale) {
   pdl_wait();
   pdl_launch_dependents();
@@ -195,10 +199,10 @@ __global__ void cutouts_aug_bwd_kernel(const __half* __restrict__ dpatch, const 
     aug_pool_bin(oy, gm.Sy, cs, ys, ye);
     aug_pool_bin(ox, gm.Sx, cs, xs, xe);
     const int patch = (oy / P) * g + (ox / P), ky = oy % P, kx = ox % P;
-    const __half* dp = dpatch + (((int64_t)k * B + b) * G2 + patch) * Kpad + ky * P + kx;
+    const InT* dp = dpatch + (((int64_t)k * B + b) * G2 + patch) * Kpad + ky * P + kx;
     // d / d I8[c] of every pixel of the bin: pooled mean, CLIP normalisation, (x + 1) / 2, the tower's gradient scale
     const float inv = 0.5f * scale / (float)((ye - ys) * (xe - xs));
-    float d[3] = {__half2float(dp[0]) * inv / stdv.x, __half2float(dp[PP]) * inv / stdv.y, __half2float(dp[2 * PP]) * inv / stdv.z};
+    float d[3] = {aug_in(dp) * inv / stdv.x, aug_in(dp + PP) * inv / stdv.y, aug_in(dp + 2 * PP) * inv / stdv.z};
     if (gm.gray) {  // I7[c] = L(I6) for every c  =>  d I6[c'] = weight[c'] * sum_c d I7[c]
       const float t = d[0] + d[1] + d[2];
       d[0] = 0.2989f * t;
@@ -262,9 +266,18 @@ int launch_cutouts_aug_bwd(const CgdOp& op, cudaStream_t st) {
   const int64_t B = op.i[0], H = op.i[1], W = op.i[2], cutn = op.i[3], cs = op.i[4], P = op.i[5], Kpad = op.i[6];
   CGD_CHECK_ARG(B > 0 && H > 0 && W > 0 && cutn > 0 && cs > 0 && P > 0 && cs % P == 0 && Kpad >= 3 * P * P, "cutouts_aug_bwd: bad dims");
   CGD_CHECK_ARG(op.p[0] && op.p[1] && op.p[2] && op.p[3], "cutouts_aug_bwd: null pointer (d_patches, coords, dx, params)");
-  CGD_CUDA(launch_pdl(cutouts_aug_bwd_kernel, dim3(aug_blocks(cutn * B * cs * cs)), dim3(256), 0, st, (const __half*)op.p[0], (const int*)op.p[1],
-                      (const float*)op.p[3], (float*)op.p[2], (int)B, (int)H, (int)W, (int)cutn, (int)cs, (int)P, (int)Kpad,
-                      make_float3(op.f[3], op.f[4], op.f[5]), op.f[6]));
+  CGD_CHECK_ARG(op.flags == 0 || op.flags == 4, "cutouts_aug_bwd: flags must be 0 (fp16 d patches) or 4 (fp32 d cutouts), got %d", op.flags);
+  if (op.flags & 4) {
+    CGD_CHECK_ARG(P == cs && Kpad == 3 * cs * cs,
+                  "cutouts_aug_bwd: flags 4 reads fp32 d cutouts [cutn*B, 3, cs, cs]: patch must equal cut_size and Kpad 3 * cut_size^2");
+    CGD_CUDA(launch_pdl(cutouts_aug_bwd_kernel<float>, dim3(aug_blocks(cutn * B * cs * cs)), dim3(256), 0, st, (const float*)op.p[0],
+                        (const int*)op.p[1], (const float*)op.p[3], (float*)op.p[2], (int)B, (int)H, (int)W, (int)cutn, (int)cs, (int)P, (int)Kpad,
+                        make_float3(op.f[3], op.f[4], op.f[5]), op.f[6]));
+  } else {
+    CGD_CUDA(launch_pdl(cutouts_aug_bwd_kernel<__half>, dim3(aug_blocks(cutn * B * cs * cs)), dim3(256), 0, st, (const __half*)op.p[0],
+                        (const int*)op.p[1], (const float*)op.p[3], (float*)op.p[2], (int)B, (int)H, (int)W, (int)cutn, (int)cs, (int)P, (int)Kpad,
+                        make_float3(op.f[3], op.f[4], op.f[5]), op.f[6]));
+  }
   CGD_LAUNCH_CHECK();
   return 0;
 }

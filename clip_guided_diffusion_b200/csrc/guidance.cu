@@ -69,8 +69,12 @@ __global__ void cutouts_fwd_kernel(const float* __restrict__ x, const int* __res
 // ---------------------------------------------------------------- cutouts backward (gather, no atomics)
 // ACC (CUTOUTS_BWD flags 2): dx += the cutout gradient instead of dx = it -- the CLIP towers of an ensemble after the first add
 // theirs in launch order.  The sum is an explicit __fadd_rn, so dx ends bitwise equal to old + what ACC = false stores.
-template <bool ACC>
-__global__ void cutouts_bwd_kernel(const __half* __restrict__ dpatch, const int* __restrict__ coords, float* __restrict__ dx, int B, int H,
+// InT = __half: the CLIP tower's patch-row gradient; float (flags 4): the stand-alone MakeCutouts backward's d cutouts
+// [cutn*B, 3, cs, cs], which is the patch layout with P = cs, Kpad = 3 cs^2.
+__device__ __forceinline__ float cut_in(const __half* p) { return __half2float(*p); }
+__device__ __forceinline__ float cut_in(const float* p) { return *p; }
+template <typename InT, bool ACC>
+__global__ void cutouts_bwd_kernel(const InT* __restrict__ dpatch, const int* __restrict__ coords, float* __restrict__ dx, int B, int H,
                                    int W, int cutn, int cs, int P, int Kpad, float3 stdv, float scale) {
   pdl_wait();
   pdl_launch_dependents();
@@ -92,7 +96,7 @@ __global__ void cutouts_bwd_kernel(const __half* __restrict__ dpatch, const int*
       // output rows whose bin [floor(o*S/cs), ceil((o+1)*S/cs)) contains ry
       const int oy0 = (int)(((unsigned)ry * (unsigned)cs) / (unsigned)Sy), oy1 = min(cs - 1, (int)((((unsigned)(ry + 1)) * (unsigned)cs + Sy - 1) / (unsigned)Sy) - 1);
       const int ox0 = (int)(((unsigned)rx * (unsigned)cs) / (unsigned)Sx), ox1 = min(cs - 1, (int)((((unsigned)(rx + 1)) * (unsigned)cs + Sx - 1) / (unsigned)Sx) - 1);
-      const __half* dp = dpatch + ((int64_t)k * B + b) * G2 * Kpad + (int64_t)c * PP;
+      const InT* dp = dpatch + ((int64_t)k * B + b) * G2 * Kpad + (int64_t)c * PP;
       for (int oy = oy0; oy <= oy1; ++oy) {
         int ys, ye;
         pool_bin(oy, Sy, cs, ys, ye);
@@ -102,7 +106,7 @@ __global__ void cutouts_bwd_kernel(const __half* __restrict__ dpatch, const int*
           pool_bin(ox, Sx, cs, xs, xe);
           if (rx < xs || rx >= xe) continue;
           const int patch = (oy / P) * g + (ox / P);
-          const float gv = __half2float(dp[(int64_t)patch * Kpad + (oy % P) * P + (ox % P)]);
+          const float gv = cut_in(dp + (int64_t)patch * Kpad + (oy % P) * P + (ox % P));
           acc += gv / (float)((ye - ys) * (xe - xs));
         }
       }
@@ -198,9 +202,9 @@ cutouts_fwd_rows_kernel(const float* __restrict__ x, const int* __restrict__ coo
 constexpr int CUT_MAX_CUTN = 128;
 constexpr int CUT_BWD_THREADS = 128;  // columns per block: H * ceil(W / 128) blocks per image keep >= 3 CTAs per SM at 256 x 256
 constexpr int CUT_MAX_ROWS = 8;  // output rows whose bins contain one input row: <= ceil(cs / S) + 1 (up-sampling 64 -> 224: 5)
-template <bool ACC>  // as cutouts_bwd_kernel
+template <typename InT, bool ACC>  // as cutouts_bwd_kernel
 __global__ void __launch_bounds__(CUT_BWD_THREADS)
-cutouts_bwd_rows_kernel(const __half* __restrict__ dpatch, const int* __restrict__ coords, float* __restrict__ dx, int B, int H, int W, int cutn,
+cutouts_bwd_rows_kernel(const InT* __restrict__ dpatch, const int* __restrict__ coords, float* __restrict__ dx, int B, int H, int W, int cutn,
                         int cs, int P, int Kpad, float3 stdv, float scale) {
   // per cutout, for image row yg: window geometry, the range [oy0, oy1] of output rows whose bins can contain it and, for the first
   // CUT_MAX_ROWS of them, the bin height (0 = the bin does not contain the row); rows beyond that (a window clipped to a sliver at
@@ -244,7 +248,7 @@ cutouts_bwd_rows_kernel(const __half* __restrict__ dpatch, const int* __restrict
       if (rx < 0 || rx >= Sx) continue;
       const int ox0 = (int)(((unsigned)rx * (unsigned)cs) / (unsigned)Sx);
       const int ox1 = min(cs - 1, (int)((((unsigned)(rx + 1)) * (unsigned)cs + Sx - 1) / (unsigned)Sx) - 1);
-      const __half* dp = dpatch + ((int64_t)k * B + b) * G2 * Kpad;
+      const InT* dp = dpatch + ((int64_t)k * B + b) * G2 * Kpad;
       for (int oy = oy0; oy <= oy1; ++oy) {
         int bh;
         if (oy - oy0 < CUT_MAX_ROWS) {
@@ -261,11 +265,11 @@ cutouts_bwd_rows_kernel(const __half* __restrict__ dpatch, const int* __restrict
           pool_bin(ox, Sx, cs, xs, xe);
           if (rx < xs || rx >= xe) continue;
           const int px = ox / P, kx = ox - px * P;
-          const __half* q = dp + (int64_t)(py * g + px) * Kpad + ky * P + kx;
+          const InT* q = dp + (int64_t)(py * g + px) * Kpad + ky * P + kx;
           const float rinv = 1.f / (float)(bh * (xe - xs));  // one reciprocal per tap instead of three divisions (<= 1 ulp apart)
-          acc[0] = fmaf(__half2float(q[0]), rinv, acc[0]);
-          acc[1] = fmaf(__half2float(q[PP]), rinv, acc[1]);
-          acc[2] = fmaf(__half2float(q[2 * PP]), rinv, acc[2]);
+          acc[0] = fmaf(cut_in(q), rinv, acc[0]);
+          acc[1] = fmaf(cut_in(q + PP), rinv, acc[1]);
+          acc[2] = fmaf(cut_in(q + 2 * PP), rinv, acc[2]);
         }
       }
     }
@@ -420,23 +424,31 @@ int launch_cutouts_fwd(const CgdOp& op, cudaStream_t st) {
   CGD_LAUNCH_CHECK();
   return 0;
 }
-int launch_cutouts_bwd(const CgdOp& op, cudaStream_t st) {
-  if (int rc = cutout_check(op)) return rc;
-  CGD_CHECK_ARG(op.flags == 0 || op.flags == 2, "cutouts_bwd: flags must be 0 (store) or 2 (accumulate), got %d", op.flags);
-  const bool acc = op.flags & 2;
+template <typename InT>
+static int cutouts_bwd_launch(const CgdOp& op, bool acc, cudaStream_t st) {
   const int64_t B = op.i[0], H = op.i[1], W = op.i[2];
   if (op.i[3] <= CUT_MAX_CUTN && op.i[4] <= 32768) {  // row-per-block gather with shared per-cutout row tables
-    CGD_CUDA(launch_pdl(acc ? cutouts_bwd_rows_kernel<true> : cutouts_bwd_rows_kernel<false>, dim3((unsigned)(B * H * ceil_div(W, CUT_BWD_THREADS))),
-                        dim3(CUT_BWD_THREADS), 0, st, (const __half*)op.p[0], (const int*)op.p[1], (float*)op.p[2],
-                        (int)B, (int)H, (int)W, (int)op.i[3], (int)op.i[4], (int)op.i[5], (int)op.i[6], make_float3(op.f[3], op.f[4], op.f[5]), op.f[6]));
+    CGD_CUDA(launch_pdl(acc ? cutouts_bwd_rows_kernel<InT, true> : cutouts_bwd_rows_kernel<InT, false>,
+                        dim3((unsigned)(B * H * ceil_div(W, CUT_BWD_THREADS))), dim3(CUT_BWD_THREADS), 0, st, (const InT*)op.p[0],
+                        (const int*)op.p[1], (float*)op.p[2], (int)B, (int)H, (int)W, (int)op.i[3], (int)op.i[4], (int)op.i[5], (int)op.i[6],
+                        make_float3(op.f[3], op.f[4], op.f[5]), op.f[6]));
     CGD_LAUNCH_CHECK();
     return 0;
   }
-  CGD_CUDA(launch_pdl(acc ? cutouts_bwd_kernel<true> : cutouts_bwd_kernel<false>, dim3(gw_blocks(B * 3 * H * W)), dim3(256), 0, st, (const __half*)op.p[0],
-                      (const int*)op.p[1], (float*)op.p[2], (int)B, (int)H, (int)W, (int)op.i[3], (int)op.i[4], (int)op.i[5], (int)op.i[6],
-                      make_float3(op.f[3], op.f[4], op.f[5]), op.f[6]));
+  CGD_CUDA(launch_pdl(acc ? cutouts_bwd_kernel<InT, true> : cutouts_bwd_kernel<InT, false>, dim3(gw_blocks(B * 3 * H * W)), dim3(256), 0, st,
+                      (const InT*)op.p[0], (const int*)op.p[1], (float*)op.p[2], (int)B, (int)H, (int)W, (int)op.i[3], (int)op.i[4], (int)op.i[5],
+                      (int)op.i[6], make_float3(op.f[3], op.f[4], op.f[5]), op.f[6]));
   CGD_LAUNCH_CHECK();
   return 0;
+}
+int launch_cutouts_bwd(const CgdOp& op, cudaStream_t st) {
+  if (int rc = cutout_check(op)) return rc;
+  CGD_CHECK_ARG(op.flags == 0 || op.flags == 2 || op.flags == 4 || op.flags == 6,
+                "cutouts_bwd: flags must be 0 (store), 2 (accumulate), 4 or 6 (the same from fp32 d cutouts), got %d", op.flags);
+  const bool f32_in = op.flags & 4;
+  CGD_CHECK_ARG(!f32_in || (op.i[5] == op.i[4] && op.i[6] == 3 * op.i[4] * op.i[4]),
+                "cutouts_bwd: flags 4 reads fp32 d cutouts [cutn*B, 3, cs, cs]: patch must equal cut_size and Kpad 3 * cut_size^2");
+  return f32_in ? cutouts_bwd_launch<float>(op, op.flags & 2, st) : cutouts_bwd_launch<__half>(op, op.flags & 2, st);
 }
 
 // ---------------------------------------------------------------- spherical distance loss + gradient

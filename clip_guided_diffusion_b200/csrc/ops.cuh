@@ -65,4 +65,8 @@ int launch_lpips_pair_fwd(const CgdOp& op, cudaStream_t st);
 int launch_lpips_loss(const CgdOp& op, cudaStream_t st);
 int launch_lpips_seed(const CgdOp& op, cudaStream_t st);
 int launch_lpips_pair_bwd(const CgdOp& op, cudaStream_t st);
+int launch_img_loss_fwd(const CgdOp& op, cudaStream_t st);
+int launch_img_loss_bwd(const CgdOp& op, cudaStream_t st);
+int launch_sph_dist_fwd(const CgdOp& op, cudaStream_t st);
+int launch_sph_dist_bwd(const CgdOp& op, cudaStream_t st);
 }  // namespace cgd

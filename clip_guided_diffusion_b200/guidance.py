@@ -64,29 +64,67 @@ class MakeCutouts(th.nn.Module):
         return self._generate_coords(side_x, side_y, cutn)
 
     def forward(self, input: th.Tensor, use_cache: bool = False, num_cutouts_override: int = None):
-        if not input.is_cuda:
-            raise _lib.CgdError("MakeCutouts.forward runs on the GPU only (no CPU fallback)")
+        """with grad mode on and ``input.requires_grad`` the result has a ``grad_fn`` whose backward is the gather transpose of the same
+        windows (CUTOUTS_BWD / CUTOUTS_AUG_BWD flags 4) and returns d / d input in input's dtype; otherwise a plain tensor"""
         B, C, H, W = input.shape
         assert C == 3
+        if not input.is_floating_point():
+            raise ValueError(f"MakeCutouts takes a floating-point image batch, got {input.dtype}")
         coords = self.coords_for(H, W, use_cache, num_cutouts_override)  # sic: (H, W) passed as (side_x, side_y), modules.py:52
-        cs = self.cut_size
-        x = input.detach().float().contiguous()
-        cdev = th.tensor(coords, dtype=th.int32, device=x.device)
-        if self.use_augs:  # the reference applies its augmentations to the raw cutout values: feed 2x - 1, mean 0 / std 1
+        cdev = th.tensor(coords, dtype=th.int32, device=input.device)
+        prm = noise = None
+        if self.use_augs:  # parameters and noise are drawn here, in the reference's order, whether or not a gradient follows
             from . import augs
-            out = th.empty(len(coords) * B, 1, 3 * cs * cs, dtype=th.float16, device=x.device)
             Smax = min(H, W)
-            noise = th.zeros(len(coords), 4, B, 3, Smax, Smax, device=x.device)
-            prm = augs.draw_aug_params(coords, B, H, W, noise_device=x.device, noise_out=noise).to(x.device)
-            _lib.run_op("CUTOUTS_AUG_FWD", i=[B, H, W, len(coords), cs, cs, 3 * cs * cs, Smax], f=[0.0, 0.0, 0.0, 1.0, 1.0, 1.0],
-                        p=[x * 2 - 1, cdev, out, prm, noise])
-            return out.view(len(coords) * B, 3, cs, cs).float()
-        # mean 0.5 / std 0.5 with the kernel's (x + 1) / 2 yield the raw pooled value; flags 1 = fp32 output like the reference's
-        # adaptive_avg_pool2d (the fused step writes fp16 straight into the CLIP tower's patch buffer instead)
-        out32 = th.empty(len(coords) * B, 3, cs, cs, dtype=th.float32, device=x.device)
-        _lib.run_op("CUTOUTS_FWD", flags=1, i=[B, H, W, len(coords), cs, cs, 3 * cs * cs], f=[0.5] * 6, p=[x, cdev, out32],
-                    what="cgd_cutouts_fwd")
-        return out32
+            noise = th.zeros(len(coords), 4, B, 3, Smax, Smax, device=input.device)
+            prm = augs.draw_aug_params(coords, B, H, W, noise_device=input.device, noise_out=noise).to(input.device)
+        if th.is_grad_enabled() and input.requires_grad:
+            return _CutoutsFunction.apply(input, cdev, self.cut_size, prm, noise)
+        return _cutouts_fwd(input.detach().float().contiguous(), cdev, self.cut_size, prm, noise)
+
+
+def _cutouts_fwd(x: th.Tensor, cdev: th.Tensor, cs: int, prm=None, noise=None) -> th.Tensor:
+    """pooled cutouts [cutn*B, 3, cs, cs] fp32 of x [B, 3, H, W] (fp32, contiguous) at the windows cdev (int32 [cutn, 3]); with ``prm``
+    (and ``noise``) the use_augs pipeline"""
+    B, _, H, W = x.shape
+    n = cdev.shape[0]
+    if prm is not None:  # the reference applies its augmentations to the raw cutout values: feed 2x - 1, mean 0 / std 1
+        out = th.empty(n * B, 1, 3 * cs * cs, dtype=th.float16, device=x.device)
+        _lib.run_op("CUTOUTS_AUG_FWD", i=[B, H, W, n, cs, cs, 3 * cs * cs, noise.shape[-1]], f=[0.0, 0.0, 0.0, 1.0, 1.0, 1.0],
+                    p=[x * 2 - 1, cdev, out, prm, noise])
+        return out.view(n * B, 3, cs, cs).float()
+    # mean 0.5 / std 0.5 with the kernel's (x + 1) / 2 yield the raw pooled value; flags 1 = fp32 output like the reference's
+    # adaptive_avg_pool2d (the fused step writes fp16 straight into the CLIP tower's patch buffer instead)
+    out32 = th.empty(n * B, 3, cs, cs, dtype=th.float32, device=x.device)
+    _lib.run_op("CUTOUTS_FWD", flags=1, i=[B, H, W, n, cs, cs, 3 * cs * cs], f=[0.5] * 6, p=[x, cdev, out32], what="cgd_cutouts_fwd")
+    return out32
+
+
+class _CutoutsFunction(th.autograd.Function):
+    """``MakeCutouts.forward`` under autograd.  Stateless: the windows (and the use_augs parameters) travel in the graph, so several calls
+    can share one backward.  The backward reads fp32 d cutouts, which is the patch layout with P = cs (flags 4): the pool gather
+    (deterministic) with std 0.5 undoing the forward's mean 0.5 / std 0.5 fold, or the use_augs scatter with scale 2 undoing its x * 2 - 1."""
+
+    @staticmethod
+    def forward(ctx, input, cdev, cs, prm, noise):
+        ctx.save_for_backward(cdev, prm)
+        ctx.geo = (tuple(input.shape), input.dtype, cs)
+        return _cutouts_fwd(input.detach().float().contiguous(), cdev, cs, prm, noise)
+
+    @staticmethod
+    @th.autograd.function.once_differentiable
+    def backward(ctx, d):
+        cdev, prm = ctx.saved_tensors
+        (B, _, H, W), dtype, cs = ctx.geo
+        dims = [B, H, W, cdev.shape[0], cs, cs, 3 * cs * cs]
+        d = d.float().contiguous()
+        if prm is None:
+            dx = th.empty(B, 3, H, W, device=d.device)
+            _lib.run_op("CUTOUTS_BWD", flags=4, i=dims, f=[0.0, 0.0, 0.0, 0.5, 0.5, 0.5, 1.0], p=[d, cdev, dx])
+        else:
+            dx = th.zeros(B, 3, H, W, device=d.device)  # the use_augs backward scatters into dx
+            _lib.run_op("CUTOUTS_AUG_BWD", flags=4, i=dims, f=[0.0, 0.0, 0.0, 1.0, 1.0, 1.0, 2.0], p=[d, cdev, dx, prm])
+        return dx.to(dtype), None, None, None, None
 
 
 class EngineModel:

@@ -136,7 +136,9 @@ enum {
   CGD_OP_CUTOUTS_FWD = 21,
   /* gather-style backward (no atomics): p0 dpatches(h) p1 coords p2 dx_in(f NCHW) ; i as fwd ; f3..5 std ; f6 scale
    * flags 0 = store into dx_in ; 2 = add to it (several CLIP towers: the first stores, the others add in launch order, so the sum is
-   * deterministic and bitwise old + the flags-0 result) ; any other flags are rejected */
+   * deterministic and bitwise old + the flags-0 result) ; any other flags are rejected
+   * flags 4 (alone or with 2): p0 is fp32 d cutouts [cutn*B, 3, cs, cs] (what CUTOUTS_FWD flags 1 writes: patch i5 == cut_size,
+   * Kpad i6 == 3 cut_size^2), the stand-alone MakeCutouts backward; still a gather, so the sum is deterministic */
   CGD_OP_CUTOUTS_BWD = 22,
   /* spherical_dist_loss + prompt weights + cutout mean, with analytic d/d(embed) (cgd/losses.py:10-14,
    * cgd/cgd.py:196-200,204; SURVEY K17).  p0 emb(f [cutn*B, D]) p1 targets(f [P,D]) p2 weights(f [P])
@@ -227,7 +229,8 @@ enum {
    * CLIP_NORMALIZE, one gather launch; like CUTOUTS_FWD plus p3 params(f [cutn,20]: flip | inverse affine matrix[6] | perspective on |
    * coefficients[8] | grayscale | 3 reserved -- drawn on the host in torchvision's order, clip_guided_diffusion_b200/augs.py)
    * p4 noise(f [cutn,4,B,3,Smax,Smax], the four N(0, .01^2) fields of every cutout)|0 ; i7 Smax (row stride of the noise planes).
-   * _BWD: the transposed gather scattered with fp32 atomics INTO p2 dx (zero it first: CGD_OP_FILL); p3 params; f6 gradient scale */
+   * _BWD: the transposed gather scattered with fp32 atomics INTO p2 dx (zero it first: CGD_OP_FILL); p3 params; f6 gradient scale;
+   * flags 4: p0 is fp32 d cutouts [cutn*B, 3, cs, cs] (patch i5 == cut_size, Kpad i6 == 3 cut_size^2) instead of fp16 patch rows */
   CGD_OP_CUTOUTS_AUG_FWD = 50,
   CGD_OP_CUTOUTS_AUG_BWD = 51,
   /* one axis of a separable resampling (image prompts: ResizeRight lanczos3 with antialiasing, cgd/clip_util.py:95-97), with host-built
@@ -300,6 +303,25 @@ enum {
    * p0 f0 p1 f1 p2 w(f [C]) p3 d_loss(f [B]) p4 dyn(f [N0 + N1]) p5 d f0(h [N0, HW, C])|0 p6 d f1(h [N1, HW, C])|0 ;
    * i0 B i1 HW i2 C i3 N0 i4 N1 ; flags 1 = write d f0, 2 = write d f1 (p5 / p6 set exactly for the selected sides) */
   CGD_OP_LPIPS_PAIR_BWD = 64,
+  /* The reference's tv_loss / range_loss (cgd/losses.py:5-7, 17-22) per image of x (f NCHW [B, C, H, W]) for a PyTorch cond_fn
+   * (clip_guided_diffusion_b200/losses.py): flags 1 = tv_loss (replicate pad: sum of squared right and down differences), 2 = range_loss
+   * (sum of (x - clamp(x, -1, 1))^2), each divided by C*H*W.  Two launches: a grid (nblk, B) writes each CTA's sum (fixed order) to
+   * partial[b * nblk + j], then loss[b] = the nblk partials of image b summed in order / (C*H*W).  No atomics: two runs give the same bits.
+   * p0 x p1 partial(f [B, nblk]) p2 loss(f [B]) ; i0 B i1 C i2 H i3 W i4 nblk (1..4096) */
+  CGD_OP_IMG_LOSS_FWD = 65,
+  /* dx = d_loss[b] * d loss_b / d x, one elementwise pass (flags as IMG_LOSS_FWD).  p0 x p1 d_loss(f [B]) p2 dx(f NCHW) ; i0 B i1 C i2 H i3 W */
+  CGD_OP_IMG_LOSS_BWD = 66,
+  /* spherical_dist_loss (cgd/losses.py:10-14) over a list of row pairs: out[m] = 2 asin(min(|x^ - y^| / 2, 1))^2 with
+   * x^ = x[pairs[m][0]] / max(||.||, 1e-12) and y^ = y[pairs[m][1]] likewise (F.normalize).  The host maps any broadcast of x [..., D]
+   * against y [..., D] to the pair list.  A row index out of range gives NaN.
+   * p0 x(f [Nx, D]) p1 y(f [Ny, D]) p2 pairs(i32 [M, 2]) p3 out(f [M]) ; i0 M i1 D i2 Nx i3 Ny */
+  CGD_OP_SPH_DIST_FWD = 67,
+  /* its input gradients from d_out (f [M]): every row of x (flags 1) and / or y (flags 2) sums d_out[m] * d out[m] / d row over the
+   * pairs that use it, in the order of a host-built CSR (ptr i32 [N + 1], idx i32 [M] = pair ids), then goes back through the
+   * normalisation.  A gather, no atomics.  An index out of range makes the row NaN.
+   * p0 x p1 y p2 pairs p3 d_out p4 dx(f [Nx, D])|0 p5 dy(f [Ny, D])|0 p6 x ptr|0 p7 x idx|0 p8 y ptr|0 p9 y idx|0 (set exactly for the
+   * selected sides) ; i0 M i1 D i2 Nx i3 Ny */
+  CGD_OP_SPH_DIST_BWD = 68,
   CGD_OP__COUNT
 };
 
