@@ -100,7 +100,7 @@ __global__ void maxpool2_bwd_kernel(const __half* __restrict__ dy, const __half*
 
 // One warp per pixel of one LPIPS tap.  f = features [B, HW, C] (post-ReLU), tn = normalised init-image features [Bt, HW, C]
 // (Bt = 1 broadcasts), w = lin weights [C].  xh = f / (||f|| + 1e-10); loss_b += (1 / HW) sum_p sum_c w_c (xh_c - tn_c)^2;
-// df = gscale / HW * d loss / d f, with d xh_c / d f_k = delta_ck / n - f_c f_k / (n^2 r), n = r + 1e-10, r = ||f||.
+// df = gscale / HW * d loss / d f saturated at +-60000, with d xh_c / d f_k = delta_ck / n - f_c f_k / (n^2 r), n = r + 1e-10, r = ||f||.
 __global__ void lpips_tap_kernel(const __half* __restrict__ f, const __half* __restrict__ tn, const float* __restrict__ w, __half* __restrict__ df,
                                  float* __restrict__ loss_part, int B, int64_t HW, int C, int Bt, float gscale) {
   pdl_wait();
@@ -165,7 +165,12 @@ __global__ void lpips_tap_kernel(const __half* __restrict__ f, const __half* __r
       if (v < nv) {
         float o[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = (t[k][j] * inv_n - x[k][j] * c2) * sc;
+        for (int j = 0; j < 8; ++j) {
+          // saturate like LPIPS_PAIR_BWD: at a pixel whose channels are all zero n = 1e-10 and the finite value is ~1e10 times
+          // the usual size, which fp16 would store as inf; inf and NaN pass through
+          const float u = (t[k][j] * inv_n - x[k][j] * c2) * sc;
+          o[j] = isfinite(u) ? fminf(fmaxf(u, -60000.f), 60000.f) : u;
+        }
         st8(df + pix * C + v * 8, pack8(o));
       }
     }

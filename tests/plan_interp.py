@@ -180,7 +180,7 @@ class Interp:
 
     def op_RELU_BWD(self, op):
         n = op.i[0]
-        r = self.flat(op.p[0], n).float() * (self.flat(op.p[1], n).float() > 0)
+        r = th.where(self.flat(op.p[1], n).float() > 0, self.flat(op.p[0], n).float(), th.zeros(()))
         dx = self.flat(op.p[2], n)
         dx.copy_(dx.float() + r if op.flags & 2 else r)
 
@@ -202,10 +202,11 @@ class Interp:
         f = self.V(op.p[0], (B, HW, C), (HW * C, C, 1)).float().requires_grad_()
         tn = self.V(op.p[1], (Bt, HW, C), (HW * C, C, 1)).float()
         w = self.flat(op.p[2], C)
-        xh = f / (f.pow(2).sum(-1, keepdim=True).sqrt() + 1e-10)
+        xh = f / (th.linalg.vector_norm(f, dim=-1, keepdim=True) + 1e-10)  # its backward is 0 at f = 0, like the kernel's c2
         per = ((xh - tn) ** 2 * w).sum(-1).mean(-1)  # [B]
         (g,) = th.autograd.grad(per.sum(), f)
-        self.V(op.p[3], (B, HW, C), (HW * C, C, 1)).copy_(g * op.f[0])
+        g = g * op.f[0]
+        self.V(op.p[3], (B, HW, C), (HW * C, C, 1)).copy_(th.where(th.isfinite(g), g.clamp(-60000, 60000), g))
         loss = self.flat(op.p[4], B)
         loss.copy_(loss + per.detach())
 
@@ -450,16 +451,30 @@ class Interp:
         dst.add_(gx * op.f[6])  # scatter-add into a zeroed buffer (CGD_OP_FILL precedes it)
 
     def _rr_resize(self, op, crop, k):
-        """separable resample of crop [B,3,S,S] with cutout k's device tables (left, weights, taps): zero outside the crop"""
+        """separable resample of crop [B,3,S,S] with cutout k's device tables (left, weights, taps): zero outside the crop; only the
+        first T weight slots are read"""
         cs = op.i[4]
         S = crop.shape[-1]
         left = self.V(op.p[3], (op.i[3], cs), (cs, 1))[k].long()
-        w = self.V(op.p[4], (op.i[3], cs, 16), (cs * 16, 16, 1))[k]
-        idx = left[:, None] + th.arange(16)
-        wv = w * ((idx >= 0) & (idx < S))
+        T = int(self.flat(op.p[5], op.i[3])[k])
+        w = self.V(op.p[4], (op.i[3], cs, 16), (cs * 16, 16, 1))[k][:, :T]
+        idx = left[:, None] + th.arange(T)
+        wv = th.where((idx >= 0) & (idx < S), w, th.zeros(()))
         idc = idx.clamp(0, S - 1)
         rows = (crop[:, :, idc, :] * wv[None, None, :, :, None]).sum(3)      # [B,3,cs,S]
         return (rows[:, :, :, idc] * wv[None, None, None, :, :]).sum(4)      # [B,3,cs,cs]
+
+    def _rr_gather_matrix(self, op, k, S):
+        """[cs, S]: M[o, r] = w[o][r - left[o]] for the outputs o in input r's inverse range [lo, hi] -- the backward's gather"""
+        cs, Smax = op.i[4], op.i[7]
+        left = self.V(op.p[3], (op.i[3], cs), (cs, 1))[k].long()
+        w = self.V(op.p[4], (op.i[3], cs, 16), (cs * 16, 16, 1))[k]
+        inv = self.V(op.p[5], (op.i[3], Smax, 2), (Smax * 2, 2, 1))[k]
+        M = th.zeros(cs, S)
+        for r in range(S):
+            o = th.arange(int(inv[r, 0]), int(inv[r, 1]) + 1)
+            M[o, r] = w[o, r - left[o]]
+        return M
 
     def op_CUTOUTS_RR_FWD(self, op):
         B, H, W, cutn, cs, P, kpad = op.i[:7]
@@ -475,12 +490,13 @@ class Interp:
         B, H, W, cutn, cs, P, kpad = op.i[:7]
         g2 = (cs // P) ** 2
         dp = self.V(op.p[0], (cutn * B, g2, kpad), (g2 * kpad, kpad, 1)).float()
-        dimg = self._unpatchify(dp, P, cs)
+        dimg = self._unpatchify(dp, P, cs).view(cutn, B, 3, cs, cs)
         std = th.tensor(op.f[3:6]).view(1, 3, 1, 1)
-        x = th.zeros(B, 3, H, W, requires_grad=True)
-        cuts = th.cat([self._rr_resize(op, x[:, :, oy:oy + s, ox:ox + s], k) for k, (ox, oy, s) in enumerate(self._coords(op))])
-        (gx,) = th.autograd.grad(((cuts + 1) * 0.5 / std * dimg).sum(), x)
-        self.V(op.p[2], (B, 3, H, W), (3 * H * W, H * W, W, 1)).copy_(gx * op.f[6])
+        gx = th.zeros(B, 3, H, W)
+        for k, (ox, oy, s) in enumerate(self._coords(op)):
+            M = self._rr_gather_matrix(op, k, s)
+            gx[:, :, oy:oy + s, ox:ox + s] += M.t() @ dimg[k] @ M
+        self.V(op.p[2], (B, 3, H, W), (3 * H * W, H * W, W, 1)).copy_(gx * 0.5 / std * op.f[6])
 
     def op_SPHERICAL(self, op):
         cutn, B, P, D = op.i[:4]

@@ -1,6 +1,7 @@
 """Every CONV signature the shipped plans emit is a case of tests/test_gpu_conv_kernels.py.
 
-Every engine the GPU suite runs at full size is built on the CPU with seeded weights: the cfg2, cfg3 (32 cutouts), cfg4, cfg5 (+ LPIPS),
+Every engine the GPU suite runs at full size is built on the CPU with seeded weights: the cfg2, cfg3 (32 cutouts), cfg2 with progressive
+cutout counts, cfg4, cfg5 (+ LPIPS),
 default128, 64x64 and ViT-L/14@336 guided steps, the RN50 / RN50x4 / RN50x16 towers, the text towers and the image-prompt encoders.  The
 signature of each CONV op (tests/test_gpu_conv_kernels.py `conv_signature`: shape, Npad, taps, BN, splits, cluster flag, flags, operand
 presence, strides, in-place residual) is looked up in tests/conv_plan_table.py.  A plan change that introduces a launch no GPU test runs
@@ -24,10 +25,10 @@ from clip_guided_diffusion_b200._lib import OP
 from tests import test_gpu_conv_kernels as K
 
 
-def _step(size, clip, cutn, lpips=False):
+def _step(size, clip, cutn, lpips=False, **kw):
     def build(device="cpu"):
         ucfg, vcfg = pu.config_for(size, class_cond=True), pv.VIT_CONFIGS[clip]
-        extra = dict(lpips_sd=pw.seeded_lpips_state_dict(), init_scale=1000.0) if lpips else {}
+        extra = dict(lpips_sd=pw.seeded_lpips_state_dict(), init_scale=1000.0, **kw) if lpips else kw
         return pg.GuidedStepB200(ucfg, pw.seeded_state_dict(pw.unet_param_shapes(ucfg), 1234), vcfg,
                                  pw.seeded_state_dict(pw.vit_param_shapes(vcfg), 1235), device=device, batch=1, num_cutouts=cutn, **extra).plan
     return build
@@ -54,6 +55,8 @@ def _image_prompt(name):
 ENGINES = {
     "cfg2": (_step(256, "ViT-B/32", 16), {"persistent", "ws", "cluster", "narrow"}),
     "cfg3": (_step(256, "ViT-B/32", 32), {"persistent", "ws", "cluster", "narrow"}),
+    # progressive_cutout: the tower also runs at max(4, n // 4) and max(8, n // 2) cutouts (cgd/cgd.py:167-175)
+    "cfg2_progressive": (_step(256, "ViT-B/32", 16, cutn_variants=pg.CondFnB200.progressive_counts(16)[:-1]), {"persistent", "ws", "cluster", "narrow"}),
     "cfg4": (_step(512, "ViT-B/16", 16), {"persistent", "ws", "cluster", "narrow"}),
     "cfg5": (_step(512, "ViT-L/14", 64, lpips=True), {"persistent", "ws", "cluster", "narrow"}),
     "default128": (_step(128, "ViT-B/32", 16), {"persistent", "ws", "cluster", "narrow"}),

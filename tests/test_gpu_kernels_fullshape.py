@@ -6,6 +6,8 @@ Each case is a stand-alone plan.  On CUDA it runs the native kernels (`gpu` test
 CPU it runs through tests/plan_interp.py at a reduced size, which validates the references themselves on a machine without a GPU.
 The float64 references never call the interpreter's op functions.
 
+Each test runs its codes' rows of tests/op_plan_table.py -- every signature the shipped plans launch -- next to hand-written cases.
+
 Tolerances are element-wise and follow from the output dtype:
 * fp16 outputs: one fp16 ulp of the float64 value (a correctly rounded result is within half an ulp; the other half absorbs the
   fp32 arithmetic before the rounding) plus an fp32 round-off floor for values near zero, derived per op below;
@@ -26,6 +28,12 @@ from clip_guided_diffusion_b200.plan import Plan
 from clip_guided_diffusion_b200.rn import RN_CONFIGS
 from clip_guided_diffusion_b200.vit import VIT_CONFIGS
 from tests.kernel_check import D64, U, cases, check, check16, run, ulp16  # noqa: F401
+from tests.op_plan_table import rows
+
+
+def plan_id(sig):
+    """pytest id of a tests/op_plan_table.py row"""
+    return "plan-" + "-".join(str(int(v)) for v in sig)
 
 
 def fp16_values(t):
@@ -114,6 +122,7 @@ CUT_GPU = {  # name: (B, H, W, cutn, tower, extra windows)
     "B4-256-16-B32": (4, 256, 256, 16, "ViT-B/32", ()),
     "cutn160-fallback": (1, 256, 256, 160, "ViT-B/32", ()),
 }
+CUT_GPU.update({plan_id(s[:7]): (*s[:4], tuple(s[4:7]), ()) for s in rows("CUTOUTS_FWD") + rows("CUTOUTS_BWD")})
 CUT_CPU = {  # (B, H, W, cutn, (cs, P, kpad), extra windows)
     "40-5-P7-kpad": (1, 40, 40, 5, (28, 7, 192), ()),
     "up-12-P7": (1, 12, 12, 4, (28, 7, 147), ()),
@@ -190,6 +199,7 @@ SPH_GPU = {  # (cutn, B, P, D, kind)
     "16-1-17-512-negw": (16, 1, 17, 512, "random"), "64-1-65-768": (64, 1, 65, 768, "random"),
     "equal": (8, 1, 1, 512, "equal"), "179deg": (8, 1, 1, 512, "179"),
 }
+SPH_GPU.update({plan_id(s): (*s, "random") for s in rows("SPHERICAL")})
 SPH_CPU = {"4-1-1-64": (4, 1, 1, 64, "random"), "4-3-1-64": (4, 3, 1, 64, "random"), "4-1-5-64-negw": (4, 1, 5, 64, "random"),
            "equal": (3, 1, 1, 64, "equal"), "179deg": (3, 1, 1, 64, "179")}
 
@@ -309,6 +319,7 @@ def ref_guide(xin, x0, gclip, sc, tvs, rs, ss, Bg):
 
 TAIL_GPU = {f"{B}x{H}x{W}-Bg{Bg}-{r}": (B, H, W, Bg, r) for B, H, W, Bg in ((1, 256, 256, 1), (1, 512, 512, 1), (4, 256, 256, 4),
                                                                          (2, 256, 384, 2), (3, 64, 64, 8)) for r in RESPACINGS}
+TAIL_GPU.update({f"{B}x{H}x{W}-Bg{Bg}-{r}": (B, H, W, Bg, r) for B, H, W, _, Bg, _ in rows("GUIDE_GRAD") for r in RESPACINGS})
 TAIL_CPU = {f"{B}x{H}x{W}-Bg{Bg}-{r}": (B, H, W, Bg, r) for B, H, W, Bg, r in ((1, 16, 16, 1, "1000"), (2, 12, 20, 2, "ddim250"),
                                                                              (3, 8, 8, 8, "25"))}
 
@@ -408,6 +419,19 @@ def test_guidance_tail(device, case):
             assert th.equal(rd(bg2, shp), rd(bg1, shp)), f"{what}: FINAL_GRAD flags 5 + MAG_CLAMP differs from the fused clamp"
 
 
+def test_tail_cases_cover_the_plan_rows():
+    """every PMV_BLEND / GUIDE_GRAD / SEED_QUANT / FINAL_GRAD / MAG_CLAMP row of tests/op_plan_table.py is a launch of some
+    test_guidance_tail GPU case (which emits GUIDE_GRAD flags 1 with LD 64, FINAL_GRAD flags 2, 3 and 7 with dx_unet, MAG_CLAMP)"""
+    made = set()
+    for B, H, W, Bg, _ in TAIL_GPU.values():
+        HW = H * W
+        made |= {("PMV_BLEND", B, HW, 3 * B), ("GUIDE_GRAD", B, H, W, 64, Bg, 1), ("SEED_QUANT", B, HW, 64), ("MAG_CLAMP", 3 * B * HW, 3 * Bg * HW)}
+        made |= {("FINAL_GRAD", B, HW, fl, True) for fl in (2, 3, 7)}
+    for code in ("PMV_BLEND", "GUIDE_GRAD", "SEED_QUANT", "FINAL_GRAD", "MAG_CLAMP"):
+        missing = [r for r in rows(code) if (code, *r) not in made]
+        assert not missing, (code, missing)
+
+
 SQ_MAX = [2048.0, 4096.0, 2048.0 * (1 + 2.0 ** -23), 4096.0 * (1 - 2.0 ** -24), 4096.0 * (1 + 2.0 ** -23), 3000.0, 1.0, 1e-30, 3e38]
 
 
@@ -437,7 +461,7 @@ def test_seed_quant_range(device):
 
 
 # ---------------------------------------------------------------------------------------------------------------- samplers
-SAMP_GPU = {f"{r}-n{n}": (r, n) for r in RESPACINGS for n in (3 * 256 * 256,)}
+SAMP_GPU = {f"{r}-n{n}": (r, n) for r in RESPACINGS for n in sorted({3 * 256 * 256} | {s[0] for s in rows("SAMPLE_ANCESTRAL") + rows("SAMPLE_DDIM")})}
 SAMP_CPU = {f"{r}-n{n}": (r, n) for r in ("1000", "25") for n in (3 * 8 * 8,)}
 
 
@@ -506,31 +530,41 @@ def test_samplers(device, case):
 
 
 # ---------------------------------------------------------------------------------------------------------------- LayerNorm
-LN_GPU = {"800x768": (800, 768, 768), "16448x1024": (16448, 1024, 1024), "2464x512": (2464, 512, 512), "64x2048": (64, 2048, 2048),
-          "3x8": (3, 8, 8), "100x768-ldx1024": (100, 768, 1024)}
-LN_CPU = {"20x64": (20, 64, 64), "3x8": (3, 8, 8), "5x40-ldx56": (5, 40, 56), "4x2048": (4, 2048, 2048)}
+# (rows, w, ldx, ldy, ld_dy, ld_dx): LN_FWD reads i = [rows, w, ldx, ldy], LN_BWD i = [rows, w, ld_dy, ldx, ld_dx]
+LN_GPU = {k: (r, w, ldx, w, w, w) for k, (r, w, ldx) in {
+    "800x768": (800, 768, 768), "16448x1024": (16448, 1024, 1024), "2464x512": (2464, 512, 512), "64x2048": (64, 2048, 2048),
+    "3x8": (3, 8, 8), "100x768-ldx1024": (100, 768, 1024)}.items()}
+LN_GPU.update({plan_id(s): (*s, s[1], s[1]) for s in rows("LN_FWD")})
+LN_GPU.update({plan_id(s): (s[0], s[1], s[3], s[1], s[2], s[4]) for s in rows("LN_BWD")})
+LN_CPU = {"20x64": (20, 64, 64, 64, 64, 64), "3x8": (3, 8, 8, 8, 8, 8), "5x40-ldx56": (5, 40, 56, 40, 40, 40), "4x2048": (4, 2048, 2048, 2048, 2048, 2048),
+          "4x40-strided-class-rows": (4, 40, 200, 48, 40, 200)}
 
 
 @pytest.mark.parametrize("device,case", cases(LN_GPU, LN_CPU))
 def test_layernorm(device, case):
-    """CLIP's LayerNorm (fp16 in, computed in fp32, eps 1e-5) forward and backward, strided input, backward storing and accumulating"""
-    rows, w, ldx = case
+    """CLIP's LayerNorm (fp16 in, computed in fp32, eps 1e-5) forward and backward, strided input, output and gradients (ViT ln_post
+    reads the class-token rows at a stride of T * width), backward storing and accumulating"""
+    rows, w, ldx, ldy, ld_dy, ld_dx = case
     g = th.Generator().manual_seed(rows + w)
     x = (th.randn(rows, ldx, generator=g) * 2 + th.randn(rows, 1, generator=g) * 3).half()
     gamma, beta = th.randn(w, generator=g) * 0.5 + 1, th.randn(w, generator=g) * 0.2
-    dy = th.randn(rows, w, generator=g).half()
-    old = th.randn(rows, w, generator=g).half()
+    dy = th.randn(rows, ld_dy, generator=g).half()
+    old = th.randn(rows, ld_dx, generator=g).half()
     x64 = x[:, :w].to(D64)
     mean64, var64 = x64.mean(-1, keepdim=True), x64.var(-1, unbiased=False, keepdim=True)
     stats = th.cat([mean64, 1 / th.sqrt(var64 + 1e-5)], 1).float()  # the backward's input: float64 statistics rounded to fp32
     plan = Plan()
-    bx, bgm, bbt, by, bst = plan.new(rows * ldx, "h"), plan.new(w, "f"), plan.new(w, "f"), plan.new(rows * w, "h"), plan.new(2 * rows, "f")
-    bdy, bst2, bdx, bdx2 = plan.new(rows * w, "h"), plan.new(2 * rows, "f"), plan.new(rows * w, "h"), plan.new(rows * w, "h")
-    plan.emit("LN_FWD", i=[rows, w, ldx, w], f=[1e-5], p=[(bx, 0), (bgm, 0), (bbt, 0), (by, 0), (bst, 0)])
-    plan.emit("LN_BWD", i=[rows, w, w, ldx, w], p=[(bdy, 0), (bx, 0), (bgm, 0), (bst2, 0), (bdx, 0)])
-    plan.emit("LN_BWD", flags=2, i=[rows, w, w, ldx, w], p=[(bdy, 0), (bx, 0), (bgm, 0), (bst2, 0), (bdx2, 0)])
+    bx, bgm, bbt, by, bst = plan.new(rows * ldx, "h"), plan.new(w, "f"), plan.new(w, "f"), plan.new(rows * ldy, "h"), plan.new(2 * rows, "f")
+    bdy, bst2, bdx, bdx2 = plan.new(rows * ld_dy, "h"), plan.new(2 * rows, "f"), plan.new(rows * ld_dx, "h"), plan.new(rows * ld_dx, "h")
+    plan.emit("LN_FWD", i=[rows, w, ldx, ldy], f=[1e-5], p=[(bx, 0), (bgm, 0), (bbt, 0), (by, 0), (bst, 0)])
+    plan.emit("LN_BWD", i=[rows, w, ld_dy, ldx, ld_dx], p=[(bdy, 0), (bx, 0), (bgm, 0), (bst2, 0), (bdx, 0)])
+    plan.emit("LN_BWD", flags=2, i=[rows, w, ld_dy, ldx, ld_dx], p=[(bdy, 0), (bx, 0), (bgm, 0), (bst2, 0), (bdx2, 0)])
     rd = run(plan, device, [(bx, x), (bgm, gamma), (bbt, beta), (bdy, dy), (bst2, stats), (bdx, -old), (bdx2, old),
-                            (by, th.full((rows * w,), 3.0).half())])
+                            (by, th.full((rows * ldy,), 3.0).half())])
+    y_all, dx_all, dx2_all = rd(by, (rows, ldy)), rd(bdx, (rows, ld_dx)), rd(bdx2, (rows, ld_dx))
+    # the columns past w of a strided output keep what they held
+    assert bool((y_all[:, w:] == 3.0).all()) and th.equal(dx_all[:, w:], -old[:, w:]) and th.equal(dx2_all[:, w:], old[:, w:])
+    dy, old = dy[:, :w], old[:, :w]
     # forward.  Per lane w / 32 serial adds then a 5-level shuffle tree: the mean is good to n u of mean |x| and rstd to (n / 2 + 4) u
     # relatively, n = w / 32 + 5; with the affine map that is the fp32 floor next to the fp16 ulp.
     n = w / 32 + 5
@@ -539,7 +573,7 @@ def test_layernorm(device, case):
     rstd = 1 / th.sqrt(var64 + 1e-5)
     xh = (x64 - mean64) * rstd
     floor = gamma.to(D64).abs() * (rstd * n * U * x64.abs().mean(-1, keepdim=True) + xh.abs() * (n / 2 + 4) * U) + 2 * U * (ref.detach().abs() + beta.to(D64).abs())
-    check16("ln_fwd", rd(by, (rows, w)), ref.detach(), floor)
+    check16("ln_fwd", y_all[:, :w], ref.detach(), floor)
     st = rd(bst, (rows, 2)).to(D64)
     check("ln_fwd mean", st[:, :1], mean64, (n + 2) * U * x64.abs().mean(-1, keepdim=True))
     check("ln_fwd rstd", st[:, 1:], rstd, (n + 8) * U * rstd + 2 * n * U * rstd * rstd.square() * x64.abs().mean(-1, keepdim=True).square())
@@ -547,28 +581,38 @@ def test_layernorm(device, case):
     (gx,) = th.autograd.grad(ref, x64r, dy.to(D64))
     dh = dy.to(D64) * gamma.to(D64)
     mag = rstd * (dh.abs() + dh.abs().mean(-1, keepdim=True) + xh.abs() * (dh * xh).abs().mean(-1, keepdim=True))
-    check16("ln_bwd", rd(bdx, (rows, w)), gx, (n + 8) * U * mag)
-    check16("ln_bwd accumulate", rd(bdx2, (rows, w)), old.to(D64) + gx, (n + 8) * U * mag)
+    check16("ln_bwd", dx_all[:, :w], gx, (n + 8) * U * mag)
+    check16("ln_bwd accumulate", dx2_all[:, :w], old.to(D64) + gx, (n + 8) * U * mag)
 
 
 # ---------------------------------------------------------------------------------------------------------------- linear_small
 LS_MODES = [(0, 0, 0), (1, 0, 1), (0, 1, 1), (1, 1, 0), (0, 0, 1)]  # (fp16 y, accumulate, silu) for M = 1, 7, 9, 64, 65
-LS_GPU = {f"x{xd}-w{wd}-K{K}": (xd, wd, K, (1, 7, 9, 64, 65), 1000) for xd in "fh" for wd in "fh" for K in (256, 1024, 3072)}
-LS_CPU = {f"x{xd}-w{wd}-K{K}": (xd, wd, K, (1, 7, 9, 12, 17), 40) for xd in "fh" for wd in "fh" for K in (64, 96)}
+
+
+def ls_launches(xd, wd, K, Ms, N):
+    """hand-written case: one launch (M, K, N, ldx, ldy, flags, bias) per M, cycling through LS_MODES"""
+    return tuple((M, K, N, K + 8, N, silu | (2 if acc else 0) | (4 if xd == "h" else 0) | (8 if yh else 0) | (16 if wd == "h" else 0), True)
+                 for M, (yh, acc, silu) in zip(Ms, LS_MODES))
+
+
+LS_GPU = {f"x{xd}-w{wd}-K{K}": ls_launches(xd, wd, K, (1, 7, 9, 64, 65), 1000) for xd in "fh" for wd in "fh" for K in (256, 1024, 3072)}
+LS_GPU.update({plan_id(s[:6]) + ("" if s[6] else "-nobias"): (s[:7],) for s in rows("LINEAR_SMALL") if not s[7]})  # s[7]: scatter (below)
+LS_CPU = {f"x{xd}-w{wd}-K{K}": ls_launches(xd, wd, K, (1, 7, 9, 12, 17), 40) for xd in "fh" for wd in "fh" for K in (64, 96)}
+LS_CPU["nobias-yh-acc"] = ((3, 64, 24, 64, 24, 2 | 4 | 8, False),)
 
 
 @pytest.mark.parametrize("device,case", cases(LS_GPU, LS_CPU))
 def test_linear_small(device, case):
     """y (=|+=) act(x) @ W^T + b over the x / W dtype pairs, row counts across several 8-row tiles and partial ones, K up to the 96 KB
     shared-memory limit (3072 fp32 = 8 rows x 12 KB), fp32 and fp16 outputs, storing (over a poisoned output) and accumulating"""
-    xd, wd, K, Ms, N = case
-    for M, (yh, acc, silu) in zip(Ms, LS_MODES):
+    for M, K, N, ldx, ldy, flags, has_bias in case:
+        silu, acc, yh = flags & 1, bool(flags & 2), bool(flags & 8)
+        xd, wd = "h" if flags & 4 else "f", "h" if flags & 16 else "f"
         g = th.Generator().manual_seed(M * K)
-        ldx = K + 8
         x = th.randn(M, ldx, generator=g)
         Wt = th.randn(N, K, generator=g) / math.sqrt(K)
-        b = th.randn(N, generator=g) * 0.1
-        old = th.randn(M, N, generator=g)
+        b = th.randn(N, generator=g) * 0.1 if has_bias else th.zeros(N)
+        old = th.randn(M, ldy, generator=g)
         if xd == "h":
             x = x.half()
         if wd == "h":
@@ -576,10 +620,12 @@ def test_linear_small(device, case):
         if yh:
             old = old.half()
         plan = Plan()
-        bx, bw, bb, by = plan.new(M * ldx, xd), plan.new(N * K, wd), plan.new(N, "f"), plan.new(M * N, "h" if yh else "f")
-        flags = silu | (2 if acc else 0) | (4 if xd == "h" else 0) | (8 if yh else 0) | (16 if wd == "h" else 0)
-        plan.emit("LINEAR_SMALL", flags=flags, i=[M, K, N, ldx, N], p=[(bx, 0), (bw, 0), (bb, 0), (by, 0)])
+        bx, bw, bb, by = plan.new(M * ldx, xd), plan.new(N * K, wd), plan.new(N, "f"), plan.new(M * ldy, "h" if yh else "f")
+        plan.emit("LINEAR_SMALL", flags=flags, i=[M, K, N, ldx, ldy], p=[(bx, 0), (bw, 0), (bb, 0) if has_bias else None, (by, 0)])
         rd = run(plan, device, [(bx, x), (bw, Wt), (bb, b), (by, old)])
+        y_all = rd(by, (M, ldy))
+        assert th.equal(y_all[:, N:], old[:, N:]), "linear_small wrote past N"
+        old = old[:, :N]
         xa = x[:, :K].to(D64)
         mag_x = xa.abs()
         if silu:
@@ -593,14 +639,33 @@ def test_linear_small(device, case):
         if silu:
             mag = mag + 2.0 ** -12 * (mag_x @ Wt.to(D64).abs().t()) if device == "cuda" else mag
         what = f"linear_small M={M} K={K} x{xd} w{wd} y{'h' if yh else 'f'} acc={acc} silu={silu}"
-        got = rd(by, (M, N))
+        got = y_all[:, :N]
         if yh:
             check16(what, got, ref, mag)
         else:
             check(what, got, ref, mag)
 
 
-@pytest.mark.parametrize("device,B,size", [pytest.param("cuda", 4, 256, marks=pytest.mark.gpu, id="gpu-256-B4"), pytest.param("cpu", 1, 64, id="cpu-64-B1")])
+def emb_layers_cases():
+    """(B, image size) of every scattering LINEAR_SMALL row of tests/op_plan_table.py (M = B, K = 4 model_channels, N = the sum of the
+    ResBlocks' 2 Cout), and B = 4 at 256"""
+    from clip_guided_diffusion_b200.unet import config_for
+    from clip_guided_diffusion_b200.weights import unet_param_shapes
+    geo = {}
+    for size in (64, 128, 256, 512):
+        cfg = config_for(size)
+        n = sum(v[0] for k, v in unet_param_shapes(cfg).items() if ".emb_layers." in k and k.endswith(".weight"))
+        geo[(4 * cfg.model_channels, n)] = size
+    out = {(4, 256)}
+    for s in rows("LINEAR_SMALL"):
+        if s[7]:
+            assert (s[1], s[2]) in geo, f"scattering LINEAR_SMALL {s} is no UNet's emb_layers"
+            out.add((s[0], geo[(s[1], s[2])]))
+    return sorted(out)
+
+
+@pytest.mark.parametrize("device,B,size", [pytest.param("cuda", B, size, marks=pytest.mark.gpu, id=f"gpu-{size}-B{B}") for B, size in emb_layers_cases()]
+                         + [pytest.param("cpu", 1, 64, id="cpu-64-B1")])
 def test_linear_small_emb_layers_scatter(device, B, size):
     """The UNet prelude's fused emb_layers launch -- one LINEAR_SMALL scattering into every ResBlock's scale-shift buffer through the
     column table -- as the UNet builder emits it (unet.emit_emb_layers), over random fp16-valued emb_layers weights"""
@@ -641,13 +706,13 @@ def ref_timestep_embedding(timesteps, dim, max_period=10000):
 
 
 @pytest.mark.parametrize("device", [pytest.param("cuda", marks=pytest.mark.gpu), "cpu"])
-@pytest.mark.parametrize("dim", [256, 1024])
+@pytest.mark.parametrize("B,dim", [pytest.param(B, d, id=str(d) if B == 4 else f"B{B}-{d}")
+                                   for B, d in sorted({(4, 256), (4, 1024)} | set(rows("TIMESTEP_EMB")))])
 @pytest.mark.parametrize("tscale", [1.0, 1000.0 / 250])
-def test_timestep_emb(device, dim, tscale):
-    """t in {0, 1, 499, 999} times the rescale factor: arguments up to ~4000 rad.  The frequencies may differ from torch's by 2 ulps
-    (expf), which moves an argument by 2 u |arg|: the tolerance is 8 u |t freq| + 4 u absolute (|cos|, |sin| <= 1)."""
-    t = th.tensor([0.0, 1.0, 499.0, 999.0])
-    B = t.numel()
+def test_timestep_emb(device, B, dim, tscale):
+    """t in {999, 0, 1, 499} (the first B) times the rescale factor: arguments up to ~4000 rad.  The frequencies may differ from
+    torch's by 2 ulps (expf), which moves an argument by 2 u |arg|: the tolerance is 8 u |t freq| + 4 u absolute (|cos|, |sin| <= 1)."""
+    t = th.tensor([999.0, 0.0, 1.0, 499.0])[:B]
     plan = Plan()
     bt, bo = plan.new(B, "f"), plan.new(B * dim, "f")
     plan.emit("TIMESTEP_EMB", i=[B, dim], f=[tscale], p=[(bt, 0), (bo, 0)])
@@ -660,13 +725,14 @@ def test_timestep_emb(device, dim, tscale):
     check(f"timestep_emb dim={dim} x{tscale}", rd(bo, (B, dim)), ref.to(D64), 8 * U * arg + 4 * U)
 
 
-@pytest.mark.parametrize("device", [pytest.param("cuda", marks=pytest.mark.gpu), "cpu"])
-def test_label_add(device):
+@pytest.mark.parametrize("device,B,D", [pytest.param("cuda", 4, 1024, marks=pytest.mark.gpu, id="cuda"), pytest.param("cpu", 4, 1024, id="cpu")]
+                         + [pytest.param("cuda", B, D, marks=pytest.mark.gpu, id=f"cuda-{plan_id((B, D))}") for B, D in rows("LABEL_ADD")])
+def test_label_add(device, B, D):
     """emb += label_emb.weight[y]: one fp32 add, bitwise"""
-    B, D, NC = 4, 1024, 1000
+    NC = 1000
     g = th.Generator().manual_seed(0)
     emb, table = th.randn(B, D, generator=g), th.randn(NC, D, generator=g)
-    y = th.tensor([0, 999, 7, 999], dtype=th.int64)
+    y = th.tensor([999, 0, 7, 999], dtype=th.int64)[:B]
     plan = Plan()
     be, bt, by = plan.new(B * D, "f"), plan.new(NC * D, "f"), plan.new(B, "i64")
     plan.emit("LABEL_ADD", i=[B, D], p=[(be, 0), (bt, 0), (by, 0)])
@@ -675,6 +741,7 @@ def test_label_add(device):
 
 
 VIT_GPU = {"B32-T50": (16, "ViT-B/32"), "B16-T197": (16, "ViT-B/16"), "L14-T257": (64, "ViT-L/14"), "L14-336-T577": (8, "ViT-L/14@336px")}
+VIT_GPU.update({plan_id(s): (s[0], tuple(s[1:])) for s in rows("VIT_EMBED")})
 VIT_CPU = {"T10-w32": (3, (10, 32)), "T5-w8": (2, (5, 8))}
 
 
@@ -703,6 +770,7 @@ def test_vit_embed(device, case):
 
 
 AP_GPU = {"RN50-49x2048": (16, 49, 2048, 2048), "RN50x16-144x3072-ld": (8, 144, 3072, 3136)}
+AP_GPU.update({plan_id(s[:4]): tuple(s[:4]) for s in rows("ATTNPOOL_EMBED_FWD") + rows("ATTNPOOL_EMBED_BWD")})
 AP_CPU = {"9x64": (3, 9, 64, 64), "4x16-ld": (2, 4, 16, 24)}
 
 
@@ -738,7 +806,9 @@ def test_attnpool_embed(device, case):
     check16(f"attnpool_embed_bwd accumulate HW={HW}", rd(bdx2, (n, HW, ld))[..., :C], gref + old[..., :C].to(D64), floor + 2 * U * old[..., :C].to(D64).abs())
 
 
-@pytest.mark.parametrize("device,n", [pytest.param("cuda", 1 << 20, marks=pytest.mark.gpu, id="gpu"), pytest.param("cpu", 4096, id="cpu")])
+@pytest.mark.parametrize("device,n", [pytest.param("cuda", n, marks=pytest.mark.gpu, id="gpu" if n == 1 << 20 else f"gpu-{n}")
+                                      for n in sorted({1 << 20} | {s[0] for s in rows("QGELU_FWD") + rows("QGELU_BWD")})]
+                         + [pytest.param("cpu", 4096, id="cpu")])
 def test_qgelu(device, n):
     """CLIP QuickGELU a = u sigmoid(1.702 u) and its derivative on fp16 inputs over [-70, 70] including |u| >= 60, where exp(-1.702 u)
     overflows fp32: one fp16 ulp plus the subnormal spacing"""
