@@ -26,7 +26,8 @@ Several CLIP towers (``clip_model_name=["ViT-B/32", "ViT-B/16", "RN50"]``) guide
 ``num_cutouts`` windows at its own resolution, gets its own text and image targets, and the CLIP losses are summed (the reference's CLIP
 block once per tower; tv / range / sat / LPIPS once).  A name is a tower name or a path to a CLIP checkpoint file (``.pt``: a TorchScript
 archive or a plain state_dict, the architecture read from its keys).  With several towers, ``target_embeds=`` is one ``[P, D_m]`` tensor
-per tower and ``clip_state_dict=`` one state_dict (or None) per tower; ``use_augs`` and ``cutout_resize="lanczos3"`` take one tower.
+per tower and ``clip_state_dict=`` one state_dict (or None) per tower; ``use_augs`` and ``cutout_resize="lanczos3"`` take one tower.  ``cutout_resize="lanczos3"``
+(ResizeRight instead of adaptive_avg_pool2d) combines with ``height_offset`` / ``width_offset``, ``progressive_cutout`` and ``use_augs``.
 """
 from __future__ import annotations
 

@@ -286,15 +286,22 @@ cutouts_bwd_rows_kernel(const InT* __restrict__ dpatch, const int* __restrict__ 
 }
 
 // ---------------------------------------------------------------- cutouts, ResizeRight (lanczos3, antialiased) mode
-// Same contract as cutouts_fwd / cutouts_bwd, but every square S x S crop is resampled to cs x cs with the separable tables the
-// host builds per crop size (clip_guided_diffusion_b200/resize_right.py, following cgd/ResizeRight/resize_right.py:31-122):
-// left[k][o] = first input index (relative to the crop) of output o, w[k][o][0..T) its normalised weights, samples outside
-// the crop are zero (pad_mode 'constant').  inv[k][r] = [lo, hi]: the outputs whose field of view contains input r.
+// Same operands as cutouts_fwd / cutouts_bwd, but every crop -- Sy x Sx after the border clip of the reference's slicing, S x S
+// inside the image -- is resampled to cs x cs with the separable tables the host builds per crop extent
+// (clip_guided_diffusion_b200/resize_right.py, following cgd/ResizeRight/resize_right.py:31-122): left[k][o] = first input index
+// (relative to the crop) of output o, w[k][o][0..T) its normalised weights, samples outside the crop are zero (pad_mode
+// 'constant').  inv[k][r] = [lo, hi]: the outputs whose field of view contains input r.  One table set serves both axes of a square
+// crop; flags RR_XTABLES adds the x axis's own set (rectangular crops).  flags RR_CROP (use_augs): the source is the augmented crop
+// CUTOUTS_AUG_FWD flags 1 wrote, fp32 [cutn, B, 3, Smax, Smax] in [0, 1] with its origin at 0, and the backward stores d crop there
+// instead of gathering into the image (CUTOUTS_AUG_BWD flags 1 scatters it on through the augmentations).
 constexpr int RR_TMAX = 16;
+constexpr int RR_XTABLES = 1, RR_CROP = 2;
 
+template <bool CROP>
 __global__ void cutouts_rr_fwd_kernel(const float* __restrict__ x, const int* __restrict__ coords, const int* __restrict__ left,
-                                      const float* __restrict__ wt, const int* __restrict__ taps, __half* __restrict__ out, int B, int H, int W,
-                                      int cutn, int cs, int P, int Kpad, float3 mean, float3 stdv) {
+                                      const float* __restrict__ wt, const int* __restrict__ taps, const int* __restrict__ leftx,
+                                      const float* __restrict__ wtx, const int* __restrict__ tapsx, __half* __restrict__ out, int B, int H,
+                                      int W, int cutn, int cs, int P, int Kpad, int Smax, float3 mean, float3 stdv) {
   pdl_wait();
   pdl_launch_dependents();
   const int g = cs / P, G2 = g * g, PP = P * P;
@@ -311,31 +318,54 @@ __global__ void cutouts_rr_fwd_kernel(const float* __restrict__ x, const int* __
     }
     const int c = kk / PP, ky = (kk % PP) / P, kx = kk % P;
     const int oy = (patch / g) * P + ky, ox = (patch % g) * P + kx;
-    const int offx = coords[k * 3 + 0], offy = coords[k * 3 + 1], S = coords[k * 3 + 2], T = taps[k];
-    const int ly = left[k * cs + oy], lx = left[k * cs + ox];
+    const int offx = coords[k * 3 + 0], offy = coords[k * 3 + 1], S = coords[k * 3 + 2];
+    const int Sy = min(S, H - offy), Sx = min(S, W - offx), Ty = taps[k], Tx = tapsx[k];
+    const int ly = left[k * cs + oy], lx = leftx[k * cs + ox];
     const float* wy = wt + ((int64_t)k * cs + oy) * RR_TMAX;
-    const float* wx = wt + ((int64_t)k * cs + ox) * RR_TMAX;
-    const float* src = x + ((int64_t)b * 3 + c) * H * W;
+    const float* wx = wtx + ((int64_t)k * cs + ox) * RR_TMAX;
+    const float* src = CROP ? x + (((int64_t)k * B + b) * 3 + c) * Smax * Smax : x + ((int64_t)b * 3 + c) * H * W + (int64_t)offy * W + offx;
+    const int ld = CROP ? Smax : W;
     float acc = 0.f;
-    for (int i = 0; i < T; ++i) {
+    for (int i = 0; i < Ty; ++i) {
       const int yy = ly + i;
-      if (yy < 0 || yy >= S) continue;
-      const float* row = src + (int64_t)(offy + yy) * W + offx;
+      if (yy < 0 || yy >= Sy) continue;
+      const float* row = src + (int64_t)yy * ld;
       float rs = 0.f;
-      for (int j = 0; j < T; ++j) {
+      for (int j = 0; j < Tx; ++j) {
         const int xx = lx + j;
-        if (xx >= 0 && xx < S) rs = fmaf(wx[j], row[xx], rs);
+        if (xx >= 0 && xx < Sx) rs = fmaf(wx[j], row[xx], rs);
       }
       acc = fmaf(wy[i], rs, acc);
     }
     const float mu = c == 0 ? mean.x : (c == 1 ? mean.y : mean.z);
     const float sd = c == 0 ? stdv.x : (c == 1 ? stdv.y : stdv.z);
-    out[idx] = __float2half_rn(((acc + 1.f) * 0.5f - mu) / sd);
+    out[idx] = __float2half_rn(CROP ? (acc - mu) / sd : ((acc + 1.f) * 0.5f - mu) / sd);
   }
 }
 
+// acc += d resampled crop k / d crop(ry, rx) . dp: the outputs of ry's and rx's inverse ranges, their weights at ry and rx
+__device__ __forceinline__ void rr_gather(const __half* __restrict__ dp, int k, int ry, int rx, const int* __restrict__ left,
+                                          const float* __restrict__ wt, const int* __restrict__ inv, const int* __restrict__ leftx,
+                                          const float* __restrict__ wtx, const int* __restrict__ invx, int cs, int P, int g, int Kpad, int Smax,
+                                          float& acc) {
+  const int oy0 = inv[((int64_t)k * Smax + ry) * 2], oy1 = inv[((int64_t)k * Smax + ry) * 2 + 1];
+  const int ox0 = invx[((int64_t)k * Smax + rx) * 2], ox1 = invx[((int64_t)k * Smax + rx) * 2 + 1];
+  for (int oy = oy0; oy <= oy1; ++oy) {
+    const float wyv = wt[((int64_t)k * cs + oy) * RR_TMAX + (ry - left[k * cs + oy])];
+    float rs = 0.f;
+    for (int ox = ox0; ox <= ox1; ++ox) {
+      const float wxv = wtx[((int64_t)k * cs + ox) * RR_TMAX + (rx - leftx[k * cs + ox])];
+      const int patch = (oy / P) * g + (ox / P);
+      rs = fmaf(wxv, __half2float(dp[(int64_t)patch * Kpad + (oy % P) * P + (ox % P)]), rs);
+    }
+    acc = fmaf(wyv, rs, acc);
+  }
+}
+
+// image-space gather (no atomics): one thread per pixel of dx, summing over every crop that holds it
 __global__ void cutouts_rr_bwd_kernel(const __half* __restrict__ dpatch, const int* __restrict__ coords, const int* __restrict__ left,
-                                      const float* __restrict__ wt, const int* __restrict__ inv, float* __restrict__ dx, int B, int H, int W,
+                                      const float* __restrict__ wt, const int* __restrict__ inv, const int* __restrict__ leftx,
+                                      const float* __restrict__ wtx, const int* __restrict__ invx, float* __restrict__ dx, int B, int H, int W,
                                       int cutn, int cs, int P, int Kpad, int Smax, float3 stdv, float scale) {
   pdl_wait();
   pdl_launch_dependents();
@@ -352,43 +382,77 @@ __global__ void cutouts_rr_bwd_kernel(const __half* __restrict__ dpatch, const i
     for (int k = 0; k < cutn; ++k) {
       const int offx = coords[k * 3 + 0], offy = coords[k * 3 + 1], S = coords[k * 3 + 2];
       const int ry = yg - offy, rx = xg - offx;
-      if (ry < 0 || ry >= S || rx < 0 || rx >= S) continue;
-      const int oy0 = inv[((int64_t)k * Smax + ry) * 2], oy1 = inv[((int64_t)k * Smax + ry) * 2 + 1];
-      const int ox0 = inv[((int64_t)k * Smax + rx) * 2], ox1 = inv[((int64_t)k * Smax + rx) * 2 + 1];
-      const __half* dp = dpatch + ((int64_t)k * B + b) * G2 * Kpad + (int64_t)c * PP;
-      for (int oy = oy0; oy <= oy1; ++oy) {
-        const float wyv = wt[((int64_t)k * cs + oy) * RR_TMAX + (ry - left[k * cs + oy])];
-        float rs = 0.f;
-        for (int ox = ox0; ox <= ox1; ++ox) {
-          const float wxv = wt[((int64_t)k * cs + ox) * RR_TMAX + (rx - left[k * cs + ox])];
-          const int patch = (oy / P) * g + (ox / P);
-          rs = fmaf(wxv, __half2float(dp[(int64_t)patch * Kpad + (oy % P) * P + (ox % P)]), rs);
-        }
-        acc = fmaf(wyv, rs, acc);
-      }
+      if (ry < 0 || ry >= min(S, H - offy) || rx < 0 || rx >= min(S, W - offx)) continue;
+      rr_gather(dpatch + ((int64_t)k * B + b) * G2 * Kpad + (int64_t)c * PP, k, ry, rx, left, wt, inv, leftx, wtx, invx, cs, P, g, Kpad, Smax,
+                acc);
     }
     dx[idx] = acc * (0.5f / sd) * scale;
   }
 }
 
+// crop-space gather (RR_CROP): one thread per element of d crop [cutn, B, 3, Smax, Smax]; elements outside Sy x Sx are not written
+__global__ void cutouts_rr_bwd_crop_kernel(const __half* __restrict__ dpatch, const int* __restrict__ coords, const int* __restrict__ left,
+                                           const float* __restrict__ wt, const int* __restrict__ inv, const int* __restrict__ leftx,
+                                           const float* __restrict__ wtx, const int* __restrict__ invx, float* __restrict__ dcrop, int B, int H,
+                                           int W, int cutn, int cs, int P, int Kpad, int Smax, float3 stdv, float scale) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int g = cs / P, G2 = g * g, PP = P * P;
+  const int64_t total = (int64_t)cutn * B * 3 * Smax * Smax;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int rx = (int)(idx % Smax);
+    int64_t r = idx / Smax;
+    const int ry = (int)(r % Smax);
+    r /= Smax;
+    const int c = (int)(r % 3);
+    r /= 3;
+    const int b = (int)(r % B), k = (int)(r / B);
+    const int offx = coords[k * 3 + 0], offy = coords[k * 3 + 1], S = coords[k * 3 + 2];
+    if (ry >= min(S, H - offy) || rx >= min(S, W - offx)) continue;
+    const float sd = c == 0 ? stdv.x : (c == 1 ? stdv.y : stdv.z);
+    float acc = 0.f;
+    rr_gather(dpatch + ((int64_t)k * B + b) * G2 * Kpad + (int64_t)c * PP, k, ry, rx, left, wt, inv, leftx, wtx, invx, cs, P, g, Kpad, Smax, acc);
+    dcrop[idx] = acc * (1.f / sd) * scale;
+  }
+}
+
+// the x-axis tables: p6.. with RR_XTABLES, else the y axis's (square crops)
+static int rr_tables(const CgdOp& op, const char* what, const void* const*& xt) {
+  CGD_CHECK_ARG((op.flags & ~(RR_XTABLES | RR_CROP)) == 0, "%s: unknown flags %d (1 = x-axis tables p6..p8, 2 = augmented-crop workspace)",
+                what, op.flags);
+  CGD_CHECK_ARG(op.p[3] && op.p[4] && op.p[5], "%s: null table pointer", what);
+  if (op.flags & RR_XTABLES) CGD_CHECK_ARG(op.p[6] && op.p[7] && op.p[8], "%s: flags 1 needs the x-axis tables p6..p8", what);
+  xt = (op.flags & RR_XTABLES) ? (const void* const*)&op.p[6] : (const void* const*)&op.p[3];
+  return 0;
+}
+
 static int cutout_check(const CgdOp& op);
 int launch_cutouts_rr_fwd(const CgdOp& op, cudaStream_t st) {
   if (int rc = cutout_check(op)) return rc;
-  const int64_t B = op.i[0], cutn = op.i[3], cs = op.i[4], P = op.i[5], Kpad = op.i[6];
-  CGD_CHECK_ARG(op.p[3] && op.p[4] && op.p[5], "cutouts_rr_fwd: null table pointer");
+  const void* const* xt;
+  if (int rc = rr_tables(op, "cutouts_rr_fwd", xt)) return rc;
+  const int64_t B = op.i[0], H = op.i[1], W = op.i[2], cutn = op.i[3], cs = op.i[4], P = op.i[5], Kpad = op.i[6];
+  const bool crop = op.flags & RR_CROP;
+  const int64_t Smax = crop ? op.i[7] : 0;
+  if (crop) CGD_CHECK_ARG(Smax >= std::min(H, W) && Smax <= 16384, "cutouts_rr_fwd: flags 2 needs i7 Smax >= min(H, W)");
   const int64_t total = cutn * B * (cs / P) * (cs / P) * Kpad;
-  CGD_CUDA(launch_pdl(cutouts_rr_fwd_kernel, dim3(gw_blocks(total)), dim3(256), 0, st, (const float*)op.p[0], (const int*)op.p[1], (const int*)op.p[3],
-                      (const float*)op.p[4], (const int*)op.p[5], (__half*)op.p[2], (int)B, (int)op.i[1], (int)op.i[2], (int)cutn, (int)cs, (int)P,
-                      (int)Kpad, make_float3(op.f[0], op.f[1], op.f[2]), make_float3(op.f[3], op.f[4], op.f[5])));
+  CGD_CUDA(launch_pdl(crop ? cutouts_rr_fwd_kernel<true> : cutouts_rr_fwd_kernel<false>, dim3(gw_blocks(total)), dim3(256), 0, st,
+                      (const float*)op.p[0], (const int*)op.p[1], (const int*)op.p[3], (const float*)op.p[4], (const int*)op.p[5],
+                      (const int*)xt[0], (const float*)xt[1], (const int*)xt[2], (__half*)op.p[2], (int)B, (int)H, (int)W, (int)cutn, (int)cs,
+                      (int)P, (int)Kpad, (int)Smax, make_float3(op.f[0], op.f[1], op.f[2]), make_float3(op.f[3], op.f[4], op.f[5])));
   return 0;
 }
 int launch_cutouts_rr_bwd(const CgdOp& op, cudaStream_t st) {
   if (int rc = cutout_check(op)) return rc;
-  const int64_t B = op.i[0], H = op.i[1], W = op.i[2], Smax = op.i[7];
-  CGD_CHECK_ARG(op.p[3] && op.p[4] && op.p[5] && Smax > 0, "cutouts_rr_bwd: null table pointer / Smax");
-  CGD_CUDA(launch_pdl(cutouts_rr_bwd_kernel, dim3(gw_blocks(B * 3 * H * W)), dim3(256), 0, st, (const __half*)op.p[0], (const int*)op.p[1],
-                      (const int*)op.p[3], (const float*)op.p[4], (const int*)op.p[5], (float*)op.p[2], (int)B, (int)H, (int)W, (int)op.i[3],
-                      (int)op.i[4], (int)op.i[5], (int)op.i[6], (int)Smax, make_float3(op.f[3], op.f[4], op.f[5]), op.f[6]));
+  const void* const* xt;
+  if (int rc = rr_tables(op, "cutouts_rr_bwd", xt)) return rc;
+  const int64_t B = op.i[0], H = op.i[1], W = op.i[2], cutn = op.i[3], Smax = op.i[7];
+  CGD_CHECK_ARG(Smax >= std::min(H, W) && Smax <= 16384, "cutouts_rr_bwd: i7 Smax must cover min(H, W)");
+  const bool crop = op.flags & RR_CROP;
+  CGD_CUDA(launch_pdl(crop ? cutouts_rr_bwd_crop_kernel : cutouts_rr_bwd_kernel, dim3(gw_blocks(crop ? cutn * B * 3 * Smax * Smax : B * 3 * H * W)),
+                      dim3(256), 0, st, (const __half*)op.p[0], (const int*)op.p[1], (const int*)op.p[3], (const float*)op.p[4],
+                      (const int*)op.p[5], (const int*)xt[0], (const float*)xt[1], (const int*)xt[2], (float*)op.p[2], (int)B, (int)H, (int)W,
+                      (int)cutn, (int)op.i[4], (int)op.i[5], (int)op.i[6], (int)Smax, make_float3(op.f[3], op.f[4], op.f[5]), op.f[6]));
   return 0;
 }
 

@@ -243,12 +243,13 @@ def clip_tower(cfg, state_dict, **kw):
 
 class _Tower:
     """one CLIP tower of the engine: its config, the buffers of its cutout windows (``coords``) and targets, the slot of its CLIP loss, one tower instance
-    per cutout count, and the ResizeRight tables of its windows"""
+    per cutout count, and the ResizeRight tables of its windows (``rr``: the y axis's, which serve the x axis too on a square image;
+    ``rr_x``: the x axis's own on a non-square image, else None)"""
 
     def __init__(self, cfg, tag, cutn, coords, targets, loss):
         self.cfg, self.tag, self.cutn, self.coords, self.targets, self.loss = cfg, tag, cutn, coords, targets, loss
         self.by_count = {}
-        self.rr = None  # ResizeRight: (left [cutn, cs], weights [cutn, cs, T_MAX], taps [cutn], inverse [cutn, H, 2])
+        self.rr = self.rr_x = None  # ResizeRight, per axis: (left [cutn, cs], weights [cutn, cs, T_MAX], taps [cutn], inverse [cutn, min(H, W), 2])
 
     def sfx(self, c):
         """range-mark suffix: the cutout count's ("@c", "" for the default count), then the tower's ("", "#1", "#2", ...)"""
@@ -332,10 +333,6 @@ class GuidedStepB200:
             # the vendored ResizeRight resampler north_star names (cgd/ResizeRight/resize_right.py, host tables in resize_right.py)
             if cutout_resize not in ("pool", "lanczos3"):
                 raise ValueError("cutout_resize must be 'pool' or 'lanczos3'")
-            if use_augs and cutout_resize != "pool":
-                raise NotImplementedError("use_augs runs with the reference's adaptive_avg_pool2d cutouts (cutout_resize='pool')")
-            if cutout_resize == "lanczos3" and (H != W or cutn_variants):
-                raise NotImplementedError("ResizeRight cutouts: square images and a single cutout count only")
             for c in cutn_variants:
                 if not 0 < int(c) <= cutn:
                     raise ValueError(f"cutn_variants must lie in (0, {cutn}), got {c}")
@@ -351,6 +348,8 @@ class GuidedStepB200:
                 self.aug_smax = min(H, W)
                 self.aug_prm = p.new(cutn * AUG_NP, "f", "aug_params")
                 self.aug_noise = p.new(cutn * 4 * B * 3 * self.aug_smax * self.aug_smax, "f", "aug_noise")
+                if cutout_resize == "lanczos3":  # the augmented crops ResizeRight resamples, then their gradient (one buffer, used in turn)
+                    self.aug_crop = p.new(cutn * B * 3 * self.aug_smax * self.aug_smax, "f", "aug_crop")
             for m, (cfg, sd) in enumerate(zip(cfgs, sds)):  # range marks of towers 1.. suffixed "#m", tower 0 keeps the plain ones
                 tag = f"#{m}" if m else ""
                 tw = _Tower(cfg, tag, cutn, p.new(cutn * 3, "i32", "cutout_coords" + tag), p.new(self.P * cfg.output_dim, "f", "target_embeds" + tag),
@@ -363,8 +362,12 @@ class GuidedStepB200:
                     if -(-6 * min(H, W) // cs) > T_MAX:
                         raise ValueError(f"cutout_resize='lanczos3': windows up to {min(H, W)} px down to {cs} px need {-(-6 * min(H, W) // cs)} "
                                          f"taps, the device tables hold {T_MAX} (images up to {T_MAX * cs // 6} px)")
-                    tw.rr = (p.new(cutn * cs, "i32", "rr_left"), p.new(cutn * cs * T_MAX, "f", "rr_weights"), p.new(cutn, "i32", "rr_taps"),
-                             p.new(cutn * H * 2, "i32", "rr_inverse"))
+                    # a crop is S x S inside a square image; on a non-square one the reference's slicing clips it to Sy x Sx (quirk B3), so
+                    # the x axis gets its own tables
+                    axis = lambda a: (p.new(cutn * cs, "i32", "rr_left" + a), p.new(cutn * cs * T_MAX, "f", "rr_weights" + a),  # noqa: E731
+                                      p.new(cutn, "i32", "rr_taps" + a), p.new(cutn * min(H, W) * 2, "i32", "rr_inverse" + a))
+                    tw.rr = axis("")
+                    tw.rr_x = axis("_x") if H != W else None
                 for c in sorted(counts, key=lambda v: v != cutn):  # the default count first: the others share its weights
                     tw.by_count[c] = clip_tower(cfg, sd, n_images=c * B, device=device, plan=p, parts=vit_streams, suffix=tw.sfx(c),
                                                 share=tw.by_count.get(cutn))
@@ -421,7 +424,7 @@ class GuidedStepB200:
         # slots are a ring of STAGE_SLOTS, each guarded by the event recorded after its copies were enqueued.
         staged = [self.unet.y_in, self.sc, self.unet.t_in] + ([self.aug_prm] if self.use_augs else [])
         for tw in self.towers:
-            staged += [tw.coords] + list(tw.rr or ())
+            staged += [tw.coords] + list(tw.rr or ()) + list(tw.rr_x or ())
         self._slot, size = {}, 0
         for b in staged:  # arena offset of the device buffer -> offset of its region in the slot
             self._slot[b.off], size = size, size + b.nbytes
@@ -473,9 +476,16 @@ class GuidedStepB200:
         dims, win = [B, H, W, c, cs, ps, kp], (tw.coords, 0)
         fwd_f, bwd_f = [*CLIP_MEAN, *CLIP_STD], [0, 0, 0, *CLIP_STD, 1.0 / self.vit_grad_scale]
         p.mark("cut_fwd" + sfx)
+        # ResizeRight: flags 1 = the x axis's own tables (non-square images), 2 = resample the augmented crops of aug_crop (use_augs)
+        rr_flags = (1 if tw.rr_x else 0) | (2 if self.use_augs else 0)
+        smax = min(H, W)
         if tw.rr:
-            p.emit("CUTOUTS_RR_FWD", i=dims, f=fwd_f, p=[(self.x_inb, 0), win, (vt.patches, 0), *((b, 0) for b in tw.rr[:3])],
-                   tag="make_cutouts(resize_right lanczos3)+normalize")
+            if self.use_augs:  # crop -> the torchvision pipeline at crop resolution -> ResizeRight, in the reference's order
+                p.emit("CUTOUTS_AUG_FWD", flags=1, i=dims + [smax], p=[(self.x_inb, 0), win, (self.aug_crop, 0), (self.aug_prm, 0), (self.aug_noise, 0)],
+                       tag="make_cutouts(use_augs crops)")
+            p.emit("CUTOUTS_RR_FWD", flags=rr_flags, i=dims + ([smax] if self.use_augs else []), f=fwd_f,
+                   p=[(self.aug_crop if self.use_augs else self.x_inb, 0), win, (vt.patches, 0), *((b, 0) for b in tw.rr[:3]),
+                      *((b, 0) for b in (tw.rr_x or ())[:3])], tag="make_cutouts(resize_right lanczos3)+normalize")
         elif self.use_augs:
             p.emit("CUTOUTS_AUG_FWD", i=dims + [self.aug_smax], f=fwd_f, p=[(self.x_inb, 0), win, (vt.patches, 0), (self.aug_prm, 0), (self.aug_noise, 0)],
                    tag="make_cutouts(use_augs)+normalize")
@@ -486,8 +496,13 @@ class GuidedStepB200:
                p=[(vt.embeds, 0), (tw.targets, 0), (self.weights, 0), (vt.d_embeds, 0), tw.loss], tag="spherical_dist_loss")
         p.mark("cut_bwd" + sfx)
         if tw.rr:
-            p.emit("CUTOUTS_RR_BWD", i=dims + [H], f=bwd_f, p=[(vt.d_patches, 0), win, (self.g_clip, 0), (tw.rr[0], 0), (tw.rr[1], 0), (tw.rr[3], 0)],
-                   tag="d_make_cutouts(resize_right)")
+            p.emit("CUTOUTS_RR_BWD", flags=rr_flags, i=dims + [smax], f=bwd_f,
+                   p=[(vt.d_patches, 0), win, (self.aug_crop if self.use_augs else self.g_clip, 0)]
+                   + [(b, 0) for t in (tw.rr, tw.rr_x) if t for b in (t[0], t[1], t[3])], tag="d_make_cutouts(resize_right)")
+            if self.use_augs:  # d crop -> through the augmentations, scattered into g_clip
+                p.emit("FILL", i=[B * 3 * H * W], f=[0.0], p=[(self.g_clip, 0)], tag="zero g_clip")
+                p.emit("CUTOUTS_AUG_BWD", flags=1, i=dims + [smax], f=[0, 0, 0, 1, 1, 1, 1.0], p=[(self.aug_crop, 0), win, (self.g_clip, 0), (self.aug_prm, 0)],
+                       tag="d_make_cutouts(use_augs crops)")
         elif self.use_augs:
             p.emit("FILL", i=[B * 3 * H * W], f=[0.0], p=[(self.g_clip, 0)], tag="zero g_clip")
             p.emit("CUTOUTS_AUG_BWD", i=dims, f=bwd_f, p=[(vt.d_patches, 0), win, (self.g_clip, 0), (self.aug_prm, 0)], tag="d_make_cutouts(use_augs)")
@@ -807,19 +822,22 @@ class GuidedStepB200:
         self._upload(st, self.aug_prm, prm.numel() * 4)
 
     def _stage_resize_tables(self, st, tw, windows):
-        """ResizeRight mode: per-cutout resampling tables of this step's crop sizes (cached per size on the host) -> device"""
+        """ResizeRight mode: per-cutout resampling tables of this step's crop extents (cached per extent on the host) -> device; the
+        first len(windows) rows, so every cutout count reads its own windows' tables"""
         from . import resize_right as rr
-        cs, n = tw.cfg.input_resolution, self.cutn
-        left, wts, taps, inv = tw.rr
-        pl, pw = self._region(st, left, th.int32).view(n, cs), self._region(st, wts, th.float32).view(n, cs, rr.T_MAX)
-        pt, pi_ = self._region(st, taps, th.int32), self._region(st, inv, th.int32).view(n, self.H, 2)
-        for k, (_, _, S) in enumerate(windows):
-            l, w, T = rr.tables(int(S), cs)
-            pl[k].copy_(l)
-            pw[k].copy_(w)
-            pt[k] = T
-            pi_[k, :S].copy_(rr.inverse_ranges(l, T, int(S)))
-        for b in tw.rr:
+        cs, n, smax = tw.cfg.input_resolution, self.cutn, min(self.H, self.W)
+        sets = [tw.rr] + ([tw.rr_x] if tw.rr_x else [])
+        views = [(self._region(st, l, th.int32).view(n, cs), self._region(st, w, th.float32).view(n, cs, rr.T_MAX), self._region(st, t, th.int32),
+                  self._region(st, i, th.int32).view(n, smax, 2)) for l, w, t, i in sets]
+        for k, (ox, oy, S) in enumerate(windows):
+            # the crop the reference's slicing leaves, Sy x Sx (clipped at the border, quirk B3); y tables first, then x
+            for (pl, pw, pt, pi_), ext in zip(views, (min(S, self.H - oy), min(S, self.W - ox))):
+                l, w, T = rr.tables(int(ext), cs)
+                pl[k].copy_(l)
+                pw[k].copy_(w)
+                pt[k] = T
+                pi_[k, :ext].copy_(rr.inverse_ranges(l, T, int(ext)))
+        for b in itertools.chain(*sets):
             self._upload(st, b)
 
     def fused_step(self, diffusion, mode, t_index, img, y, cond_fn, eta=0.0) -> dict:

@@ -3,7 +3,8 @@
 
 ``north_star`` names "MakeCutouts' random-crop + ResizeRight downsample"; the reference's MakeCutouts actually pools
 (cgd/modules.py:63) and only ``encode_image_prompt`` calls the vendored resampler (cgd/clip_util.py:95-97, lanczos3, antialiasing).
-This mode resizes every square crop S x S -> cut_size x cut_size exactly like
+This mode resizes every crop Sy x Sx (S x S inside the image, clipped at its border like the reference's slicing) -> cut_size x
+cut_size exactly like
 ``cgd/ResizeRight/resize_right.py:31-122`` (tensor path, pad_mode='constant', by_convs=False): for one dimension
 
     projected grid   g[o] = o / s + (S - 1) / 2 - (O - 1) / (2 s)                      (resize_right.py:126-137), s = O / S
@@ -13,7 +14,8 @@ This mode resizes every square crop S x S -> cut_size x cut_size exactly like
     out[o] = sum_i w[o, i] * in[left[o] + i], samples outside [0, S) are zero            (resize_right.py:216-247)
 
 The same float32 torch arithmetic in the same order as the reference decides the ceil() boundaries; the tables are cached per
-crop size (MakeCutouts draws S in [min(cut_size, side), side]).  Both axes of a square crop share one table.
+crop extent (MakeCutouts draws S in [min(cut_size, side), side]).  Each axis takes the table of its own extent; both axes of a square
+crop share one.
 """
 from __future__ import annotations
 

@@ -207,7 +207,13 @@ enum {
   CGD_OP_FILL = 42,
   /* MakeCutouts in ResizeRight mode (lanczos3, antialiased; cgd/ResizeRight/resize_right.py:31-122): like CUTOUTS_FWD / _BWD with
    * host-built separable tables per cutout: p3 left(i32 [cutn,cs]) p4 weights(f [cutn,cs,16]) p5 taps(i32 [cutn]) (fwd)
-   * / inverse ranges(i32 [cutn,Smax,2]) (bwd) ; i7 Smax (bwd).  Square crops only. */
+   * / inverse ranges(i32 [cutn,Smax,2]) (bwd) ; i7 Smax >= min(H, W) (bwd; fwd with flags 2).  The crop of window (ox, oy, S) is
+   * Sy x Sx = min(S, H - oy) x min(S, W - ox), as the reference's slicing clips it.  Unknown flags are rejected.
+   * flags 1: p6 left p7 weights p8 taps (fwd) / inverse ranges (bwd) of the x axis, built for Sx (p3..p5 then hold the y axis's, for
+   *   Sy); without it one table set serves both axes (square crops)
+   * flags 2 (use_augs): fwd reads p0 = the augmented crops CUTOUTS_AUG_FWD flags 1 wrote (f [cutn,B,3,Smax,Smax], values in [0, 1],
+   *   origin 0) and normalises (acc - mean) / std ; bwd stores d crop (f [cutn,B,3,Smax,Smax], Sy x Sx of each plane) into p2 instead of
+   *   gathering into dx_in, for CUTOUTS_AUG_BWD flags 1 */
   CGD_OP_CUTOUTS_RR_FWD = 43,
   CGD_OP_CUTOUTS_RR_BWD = 44,
   /* dynamic scaling of the UNet-backward seed (GUIDE_GRAD flags 1 writes the fp32 seed p7 and the per-image max |.| into p8[0..B)):
@@ -230,7 +236,10 @@ enum {
    * coefficients[8] | grayscale | 3 reserved -- drawn on the host in torchvision's order, clip_guided_diffusion_b200/augs.py)
    * p4 noise(f [cutn,4,B,3,Smax,Smax], the four N(0, .01^2) fields of every cutout)|0 ; i7 Smax (row stride of the noise planes).
    * _BWD: the transposed gather scattered with fp32 atomics INTO p2 dx (zero it first: CGD_OP_FILL); p3 params; f6 gradient scale;
-   * flags 4: p0 is fp32 d cutouts [cutn*B, 3, cs, cs] (patch i5 == cut_size, Kpad i6 == 3 cut_size^2) instead of fp16 patch rows */
+   * flags 4: p0 is fp32 d cutouts [cutn*B, 3, cs, cs] (patch i5 == cut_size, Kpad i6 == 3 cut_size^2) instead of fp16 patch rows
+   * flags 1 (ResizeRight after use_augs): _FWD writes the augmented crops themselves, f [cutn,B,3,Smax,Smax] in [0, 1] (Sy x Sx of each
+   * plane), into p2 instead of pooled patches, for CUTOUTS_RR_FWD flags 2; _BWD reads p0 = d crop in that layout (CUTOUTS_RR_BWD flags 2)
+   * and scatters it through the augmentations into p2 (f6 scale; i7 Smax) */
   CGD_OP_CUTOUTS_AUG_FWD = 50,
   CGD_OP_CUTOUTS_AUG_BWD = 51,
   /* one axis of a separable resampling (image prompts: ResizeRight lanczos3 with antialiasing, cgd/clip_util.py:95-97), with host-built
