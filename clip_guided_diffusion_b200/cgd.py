@@ -25,7 +25,10 @@ Or pass ``target_embeds`` / ``weights`` directly.  Image prompts use this packag
 Several CLIP towers (``clip_model_name=["ViT-B/32", "ViT-B/16", "RN50"]``) guide one run together: each tower cuts its own
 ``num_cutouts`` windows at its own resolution, gets its own text and image targets, and the CLIP losses are summed (the reference's CLIP
 block once per tower; tv / range / sat / LPIPS once).  A name is a tower name or a path to a CLIP checkpoint file (``.pt``: a TorchScript
-archive or a plain state_dict, the architecture read from its keys).  With several towers, ``target_embeds=`` is one ``[P, D_m]`` tensor
+archive or a plain state_dict, the architecture read from its keys).  ``"open_clip:<arch>"`` names LAION's OpenCLIP ViT towers (ViT-B-32,
+ViT-B-32-quickgelu, ViT-B-16, ViT-L-14, ViT-H-14; vit.OPEN_CLIP_CONFIGS): exact-GELU MLPs, ViT-H's 80-wide heads; weights from
+``clip_state_dict=`` or ``checkpoints_dir/open_clip/<arch>.{safetensors,bin,pt}`` (then ``CACHE_PATH/open_clip/``), checked against the
+architecture.  Their text prompts are always encoded on the device text tower (``text_encoder="clip"`` is refused for them).  With several towers, ``target_embeds=`` is one ``[P, D_m]`` tensor
 per tower and ``clip_state_dict=`` one state_dict (or None) per tower; ``use_augs`` and ``cutout_resize="lanczos3"`` take one tower.  ``cutout_resize="lanczos3"``
 (ResizeRight instead of adaptive_avg_pool2d) combines with ``height_offset`` / ``width_offset``, ``progressive_cutout`` and ``use_augs``.
 """
@@ -43,7 +46,7 @@ from .text import TextB200, text_config_from_state_dict
 from .tokenizer import find_vocab, load_tokenizer, tokenize  # noqa: F401 (tokenize: public, like clip.tokenize)
 from .unet import config_for
 from .rn import RN_CONFIGS, rn_config_from_state_dict
-from .vit import VIT_CONFIGS, vit_config_from_state_dict
+from .vit import OPEN_CLIP_CONFIGS, VIT_CONFIGS, check_open_clip_state_dict, vit_config_from_state_dict
 
 CACHE_PATH = os.path.expanduser("~/.cache/clip-guided-diffusion")  # cgd/script_util.py:18
 
@@ -154,10 +157,11 @@ def _text_encoder_choice(text_encoder, bpe_path, checkpoints_dir):
         return None
 
 
-def _encode_text_device(prompts, clip_sd, vocab, device):
-    """all text prompts in one pass of a forward-only text tower, in prompt order -> (fp32 [P, D], weights [P])"""
+def _encode_text_device(prompts, clip_sd, vocab, device, act="quick_gelu"):
+    """all text prompts in one pass of a forward-only text tower, in prompt order -> (fp32 [P, D], weights [P]); `act`: the MLP
+    activation of the tower (the visual config's, "gelu" for the OpenCLIP towers)"""
     parsed = [parse_prompt(p) for p in prompts]
-    cfg = text_config_from_state_dict(clip_sd)
+    cfg = text_config_from_state_dict(clip_sd, act=act)
     ids = load_tokenizer(vocab).tokenize([t for t, _ in parsed], context_length=cfg.context_length)
     tower = TextB200(cfg, clip_sd, len(parsed), device)
     embeds = tower.encode(ids)
@@ -171,8 +175,13 @@ def encode_text_prompt(txt: str, weight: float, clip_model_name: str = "ViT-B/32
     ``weight``), on this package's text tower: the text half of ``clip_state_dict`` or of the named checkpoint, and the BPE vocabulary
     of ``find_vocab(bpe_path, checkpoints_dir)``.  A text longer than the context raises RuntimeError like ``clip.tokenize``."""
     _require_cuda(device)
-    clip_sd = clip_state_dict if clip_state_dict is not None else _load_clip_sd(clip_model_name, checkpoints_dir)
-    embeds, _ = _encode_text_device([txt], clip_sd, find_vocab(bpe_path, checkpoints_dir), device)
+    act = "quick_gelu"
+    if open_clip_arch(clip_model_name) is not None:
+        clip_sd, cfg = _clip_tower(clip_model_name, clip_state_dict, checkpoints_dir)
+        act = cfg.act
+    else:
+        clip_sd = clip_state_dict if clip_state_dict is not None else _load_clip_sd(clip_model_name, checkpoints_dir)
+    embeds, _ = _encode_text_device([txt], clip_sd, find_vocab(bpe_path, checkpoints_dir), device, act=act)
     return embeds, weight
 
 
@@ -214,9 +223,51 @@ def _load_clip_file(path):
         return th.load(path, map_location="cpu")
 
 
+OPEN_CLIP_PREFIX = "open_clip:"
+OPEN_CLIP_SUFFIXES = (".safetensors", ".bin", ".pt")
+
+
+def open_clip_arch(clip_model_name):
+    """"open_clip:<arch>" -> arch (ValueError for an arch not in OPEN_CLIP_CONFIGS); None for any other name"""
+    name = str(clip_model_name)
+    if not name.startswith(OPEN_CLIP_PREFIX):
+        return None
+    arch = name[len(OPEN_CLIP_PREFIX):]
+    if arch not in OPEN_CLIP_CONFIGS:
+        raise ValueError(f"OpenCLIP tower {arch!r} is not supported (supported: {', '.join(OPEN_CLIP_PREFIX + a for a in OPEN_CLIP_CONFIGS)})")
+    return arch
+
+
+def open_clip_checkpoint_paths(arch, checkpoints_dir):
+    """where the weights of open_clip:<arch> are looked for, in order: checkpoints_dir/open_clip/<arch>.{safetensors,bin,pt}, then the
+    same under CACHE_PATH (the LAION hub repos' open_clip_model.safetensors / open_clip_pytorch_model.bin, renamed)"""
+    dirs = [d for d in (checkpoints_dir, CACHE_PATH) if d is not None]
+    return [os.path.join(d, "open_clip", arch + s) for d in dict.fromkeys(dirs) for s in OPEN_CLIP_SUFFIXES]
+
+
+def _load_open_clip_sd(arch, checkpoints_dir):
+    places = open_clip_checkpoint_paths(arch, checkpoints_dir)
+    path = next((p for p in places if os.path.isfile(p)), None)
+    if path is None:
+        raise FileNotFoundError(f"no weights for open_clip:{arch} in {', '.join(places)}: place the checkpoint there or pass "
+                                "clip_state_dict= (nothing is downloaded)")
+    if path.endswith(".safetensors"):
+        from safetensors.torch import load_file
+        return load_file(path, device="cpu")
+    if path.endswith(".bin"):
+        return th.load(path, map_location="cpu")
+    return _load_clip_file(path)
+
+
 def _clip_tower(clip_model_name, clip_state_dict, checkpoints_dir):
     """-> (CLIP state_dict, visual tower config): the given state_dict's own architecture, a checkpoint file's (a path) or the named
-    tower's checkpoint"""
+    tower's checkpoint.  An "open_clip:<arch>" name takes its config from OPEN_CLIP_CONFIGS, never from the keys, and the weights (given
+    or found under checkpoints_dir/open_clip/) are checked against it."""
+    arch = open_clip_arch(clip_model_name)
+    if arch is not None:
+        clip_sd = clip_state_dict if clip_state_dict is not None else _load_open_clip_sd(arch, checkpoints_dir)
+        check_open_clip_state_dict(arch, clip_sd, text="token_embedding.weight" in clip_sd)
+        return clip_sd, OPEN_CLIP_CONFIGS[arch].vision
     if clip_state_dict is None and _is_checkpoint_path(clip_model_name):
         clip_sd = _load_clip_file(str(clip_model_name))
         return clip_sd, _tower_config(clip_sd)
@@ -300,6 +351,10 @@ def clip_guided_diffusion(
         raise NotImplementedError("W&B logging is outside the hot path (SURVEY section 2)")
     if text_encoder not in ("auto", "clip", "device"):
         raise ValueError(f"text_encoder={text_encoder!r}: expected 'auto', 'clip' or 'device'")
+    open_clip = [open_clip_arch(n) is not None for n in names]  # also refuses an unknown open_clip: architecture, before any file is read
+    if text_encoder == "clip" and any(open_clip):
+        raise ValueError("text_encoder='clip' cannot encode for an open_clip: tower (the clip package does not build them): use "
+                         "text_encoder='device' or 'auto'")
     th.manual_seed(seed)
     if not use_magnitude and image_size == 64:  # cgd/cgd.py:72-74
         use_magnitude = True
@@ -312,8 +367,12 @@ def clip_guided_diffusion(
         embeds, weights = [[] for _ in towers], []
         if prompts or not image_prompts:
             vocab = _text_encoder_choice(text_encoder, bpe_path, checkpoints_dir) if prompts else None
-            for m, (name, (clip_sd, _)) in enumerate(zip(names, towers)):
-                if vocab is not None:  # one forward-only text tower from the visual tower's state_dict, released here
+            # an OpenCLIP tower always encodes on the device text tower (same BPE vocabulary); OpenAI towers keep the choice above
+            oc_vocab = find_vocab(bpe_path, checkpoints_dir) if prompts and any(open_clip) else None
+            for m, (name, (clip_sd, cfg)) in enumerate(zip(names, towers)):
+                if open_clip[m]:
+                    e, w = _encode_text_device(prompts, clip_sd, oc_vocab, device, act=cfg.act)
+                elif vocab is not None:  # one forward-only text tower from the visual tower's state_dict, released here
                     e, w = _encode_text_device(prompts, clip_sd, vocab, device)
                 else:
                     e, w = _encode_text(prompts, name, device)

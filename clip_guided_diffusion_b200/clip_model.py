@@ -95,7 +95,8 @@ class ClipModelB200:
         ids = th.as_tensor(text)
         if ids.dim() == 1:
             ids = ids[None]
-        tower = TextB200(text_config_from_state_dict(self._text_sd), self._text_sd, ids.shape[0], self.device)
+        cfg = text_config_from_state_dict(self._text_sd, act=getattr(self.cfg, "act", "quick_gelu"))  # the visual tower's MLP activation
+        tower = TextB200(cfg, self._text_sd, ids.shape[0], self.device)
         emb = tower.encode(ids)
         del tower
         return emb
@@ -180,8 +181,9 @@ def load_clip(model_name: str = "ViT-B/32", device: str = "cuda", *, max_images:
               checkpoints_dir: str = CACHE_PATH):
     """cgd/clip_util.py's ``load_clip(model_name, device) -> (clip_model, clip_size)`` on this package's towers.  ``model_name`` is a
     tower name (ViT-B/32, ViT-B/16, ViT-L/14, ViT-L/14@336px, RN50, RN101, RN50x4, RN50x16) whose checkpoint lies under
-    ``checkpoints_dir/clip/``, or a path to a CLIP checkpoint file; ``clip_state_dict=`` gives the weights directly (the architecture is
-    read from its keys).  ``max_images``: the most images one ``encode_image`` call takes (the reference's ``num_cutouts`` x batch)."""
+    ``checkpoints_dir/clip/``, an OpenCLIP tower ``"open_clip:<arch>"`` (vit.OPEN_CLIP_CONFIGS; weights under ``checkpoints_dir/open_clip/``),
+    or a path to a CLIP checkpoint file; ``clip_state_dict=`` gives the weights directly (the architecture is read from its keys, except
+    for an ``open_clip:`` name, whose architecture the weights are checked against).  ``max_images``: the most images one ``encode_image`` call takes (the reference's ``num_cutouts`` x batch)."""
     _require_cuda(device)
     sd, cfg = _clip_tower(model_name, clip_state_dict, checkpoints_dir)
     model = ClipModelB200(cfg, sd, max_images, device)

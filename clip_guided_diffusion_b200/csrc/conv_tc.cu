@@ -158,6 +158,13 @@ __device__ __forceinline__ float qgelu_grad_mul(float a, float u) {
   return a * (sg * fmaf(1.702f * u, 1.f - sg, 1.f));
 }
 
+// CONV flags 8: acc * GELU'(u) = acc * (Phi(u) + u phi(u)), the exact (erf) GELU of the OpenCLIP towers
+__device__ __forceinline__ float gelu_grad_mul(float a, float u) {
+  const float cdf = 0.5f * erfcf(u * -0.70710678118654752f);  // Phi(u) without the cancellation 1 + erf(.) has for u << 0
+  const float pdf = 0.39894228040143268f * __expf(-0.5f * u * u);
+  return a * fmaf(u, pdf, cdf);
+}
+
 template <int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvTcParams p) {
@@ -367,7 +374,8 @@ struct PersistCfg {
   }
 };
 
-template <int BN>
+// EXACT_GELU: the instantiation that runs CONV flags 8 (res_mode 2); the other one keeps its registers free of erff / expf
+template <int BN, bool EXACT_GELU = false>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                           const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmRes, const ConvTcParams p) {
@@ -505,7 +513,10 @@ conv_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
             __half2* hi = reinterpret_cast<__half2*>(box + Cfg::swz(r0 + 8, cb));
             if (p.res) {
               const float2 u0 = __half22float2(*lo), u1 = __half22float2(*hi);
-              if (p.res_mode == 1) {
+              if constexpr (EXACT_GELU) {
+                v0 = gelu_grad_mul(v0, u0.x); v1 = gelu_grad_mul(v1, u0.y);
+                v2 = gelu_grad_mul(v2, u1.x); v3 = gelu_grad_mul(v3, u1.y);
+              } else if (p.res_mode == 1) {
                 v0 = qgelu_grad_mul(v0, u0.x); v1 = qgelu_grad_mul(v1, u0.y);
                 v2 = qgelu_grad_mul(v2, u1.x); v3 = qgelu_grad_mul(v3, u1.y);
               } else {
@@ -749,13 +760,15 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
                   "conv: layer flagged for cluster split-K is not eligible (BN=%d splits=%d Cout=%d f32=%d)", L.BN, p.splits, p.Cout, p.out_f32);
     p.cluster = 1;
   }
-  // flags 4: the "residual" operand is a QuickGELU pre-activation u and the epilogue computes acc * QuickGELU'(u) instead of acc + res
+  // flags 4: the "residual" operand is a QuickGELU pre-activation u and the epilogue computes acc * QuickGELU'(u) instead of acc + res;
+  // flags 8: the same with the exact GELU'(u) = Phi(u) + u phi(u)
   p.res_mode = 0;
-  if (op.flags & 4) {
+  CGD_CHECK_ARG((op.flags & 12) != 12, "conv: flags 4 (QuickGELU') and 8 (GELU') exclude each other");
+  if (op.flags & 12) {
     CGD_CHECK_ARG(L.impl != 1 && p.splits == 1 && !p.out_f32 && p.out_sc == 1 && Cout % 8 == 0 && p.res != nullptr && p.bias == nullptr,
-                  "conv: flags 4 (QuickGELU' epilogue) needs the tensor-core kernel without split-K, an fp16 contiguous output with Cout %% 8 == 0, a res "
-                  "operand and no bias (BN=%d splits=%d Cout=%lld)", (int)BN, p.splits, (long long)Cout);
-    p.res_mode = 1;
+                  "conv: flags %d (GELU' epilogue) needs the tensor-core kernel without split-K, an fp16 contiguous output with Cout %% 8 == 0, a res "
+                  "operand and no bias (BN=%d splits=%d Cout=%lld)", op.flags & 12, (int)BN, p.splits, (long long)Cout);
+    p.res_mode = (op.flags & 4) ? 1 : 2;
   }
   // <= 8 output channels, fp32 output, 3x3 (UNet head, stem dgrad): halo-tile mma.sync kernel (conv_narrow.cu); CGD_CONV_NARROW=0 keeps
   // the wgmma N = 16 tile for A/B runs
@@ -768,6 +781,7 @@ int conv_tc_prepare(const CgdOp& op, ConvTcLaunch& L) {
     L.narrow = (narrow_on && conv_narrow_eligible(L)) ? 1 : 0;
   }
   L.persistent = (!L.narrow && p.splits == 1 && !p.cluster && !p.out_f32 && p.out_sc == 1 && p.Cout % 8 == 0) ? 1 : 0;
+  CGD_CHECK_ARG(p.res_mode != 2 || (L.persistent && BN >= 64), "conv: flags 8 (GELU' epilogue) runs on the persistent kernel with BN >= 64 (BN=%d)", (int)BN);
   if (L.persistent) {
     // output / residual boxes of the persistent epilogue: 128 pixels x min(BN, 64) channels, swizzled like the staging tile.  The C
     // extent is Cout, so the TMA unit clips padded columns and pixels outside the image; channel slices are a base pointer plus
@@ -799,6 +813,8 @@ static int set_smem_attr() {
   if (attr_set.needed()) {
     CGD_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BN>::kSmemBytes));
     CGD_CUDA(cudaFuncSetAttribute(conv_tc_persistent_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, PersistCfg<BN>::kSmemBytes));
+    if constexpr (BN >= 64)
+      CGD_CUDA(cudaFuncSetAttribute(conv_tc_persistent_kernel<BN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, PersistCfg<BN>::kSmemBytes));
     attr_set.mark();
   }
   return 0;
@@ -833,8 +849,14 @@ static int launch_tc(const ConvTcLaunch& L, cudaStream_t st) {
   }
   cfg.attrs = attrs;
   cfg.numAttrs = na;
-  if (L.persistent) CGD_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_persistent_kernel<BN>, L.tmA, L.tmB, L.tmOut, L.tmRes, L.p));
-  else CGD_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN>, L.tmA, L.tmB, L.p));
+  if (L.persistent && L.p.res_mode == 2) {
+    if constexpr (BN >= 64) CGD_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_persistent_kernel<BN, true>, L.tmA, L.tmB, L.tmOut, L.tmRes, L.p));
+    else CGD_CHECK_ARG(false, "conv: flags 8 (GELU' epilogue) needs BN >= 64, got %d", BN);
+  } else if (L.persistent) {
+    CGD_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_persistent_kernel<BN>, L.tmA, L.tmB, L.tmOut, L.tmRes, L.p));
+  } else {
+    CGD_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN>, L.tmA, L.tmB, L.p));
+  }
   return 0;
 }
 

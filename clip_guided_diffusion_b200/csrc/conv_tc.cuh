@@ -27,7 +27,8 @@ struct ConvTcParams {
   void* out;
   float* ws;                         // split-K partials [splits][m_tiles*128][Npad]
   int res_mode;                      // 0 = out = acc (+bias) + res ; 1 = out = acc * QuickGELU'(res) (CONV flags 4: the dgrad of the ViT's
-                                     // c_proj writes d(c_fc output) directly, `res` = the saved pre-activation)
+                                     // c_proj writes d(c_fc output) directly, `res` = the saved pre-activation) ; 2 = out = acc * GELU'(res)
+                                     // (CONV flags 8: the same for the exact-GELU MLPs of the OpenCLIP towers)
 };
 
 struct ConvTcLaunch {

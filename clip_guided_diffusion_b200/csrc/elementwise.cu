@@ -255,7 +255,9 @@ int launch_label_add(const CgdOp& op, cudaStream_t st) {
   return 0;
 }
 
-// ---- QuickGELU ([3P] clip.model.QuickGELU): a = u * sigmoid(1.702 u)
+// ---- QuickGELU ([3P] clip.model.QuickGELU): a = u * sigmoid(1.702 u); EXACT (QGELU_FWD flags 1, the OpenCLIP towers' nn.GELU):
+// a = 0.5 u (1 + erf(u / sqrt 2)) = 0.5 u erfc(-u / sqrt 2) in fp32 from the fp16 u, rounded once to fp16
+template <bool EXACT>
 __global__ void qgelu_fwd_kernel(const __half* __restrict__ u, __half* __restrict__ a, int64_t nvec) {
   pdl_wait();
   pdl_launch_dependents();
@@ -263,7 +265,10 @@ __global__ void qgelu_fwd_kernel(const __half* __restrict__ u, __half* __restric
     float v[8];
     unpack8(ld8(u + idx * 8), v);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = v[j] / (1.f + __expf(-1.702f * v[j]));
+    for (int j = 0; j < 8; ++j) {
+      if (EXACT) v[j] = 0.5f * v[j] * erfcf(v[j] * -0.70710678118654752f);  // Phi(u) = erfc(-u / sqrt 2) / 2: no cancellation for u << 0
+      else v[j] = v[j] / (1.f + __expf(-1.702f * v[j]));
+    }
     st8(a + idx * 8, pack8(v));
   }
 }
@@ -285,7 +290,11 @@ __global__ void qgelu_bwd_kernel(const __half* __restrict__ da, const __half* __
 int launch_qgelu_fwd(const CgdOp& op, cudaStream_t st) {
   const int64_t n = op.i[0];
   CGD_CHECK_ARG(n > 0 && n % 8 == 0 && op.p[0] && op.p[1], "qgelu: bad args");
-  CGD_CUDA(launch_pdl(qgelu_fwd_kernel, dim3(ew_blocks(n / 8)), dim3(256), 0, st, (const __half*)op.p[0], (__half*)op.p[1], n / 8));
+  CGD_CHECK_ARG((op.flags & ~1) == 0, "qgelu: unknown flags %d (1 = exact GELU)", op.flags);
+  if (op.flags & 1)
+    CGD_CUDA(launch_pdl(qgelu_fwd_kernel<true>, dim3(ew_blocks(n / 8)), dim3(256), 0, st, (const __half*)op.p[0], (__half*)op.p[1], n / 8));
+  else
+    CGD_CUDA(launch_pdl(qgelu_fwd_kernel<false>, dim3(ew_blocks(n / 8)), dim3(256), 0, st, (const __half*)op.p[0], (__half*)op.p[1], n / 8));
   CGD_LAUNCH_CHECK();
   return 0;
 }

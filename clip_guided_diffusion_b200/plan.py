@@ -229,7 +229,8 @@ class Plan:
         # 512 -> 512 and 1024 -> 512 3x3s): a wider tile split along K inside a cluster shortens the K loop per SM.
         # CGD_CLUSTER_WIDE=0 switches it off for A/B runs.
         self.cluster_wide = os.environ.get("CGD_CLUSTER_WIDE", "1") == "1"
-        self._gelu_src = {}   # QuickGELU output Act key -> its pre-activation Act (dgrad-epilogue fusion, CONV flags 4)
+        # (Quick)GELU output Act key -> (its pre-activation Act, exact GELU?) (dgrad-epilogue fusion, CONV flags 4 / 8)
+        self._gelu_src = {}
         self.arena: Optional[th.Tensor] = None
         self.handle = None
         self._c_ops = None
@@ -306,11 +307,16 @@ class Plan:
 
     # ------------------------------------------------------------------ conv / GEMM
     def _emit_conv(self, x_ptr, x_strides, NB, H, W, Cin, wbuf, npad, Cout, taps, bias, res_ptr, res_strides, out_ptr, out_strides,
-                   out_f32=False, out_sc=1, tag="", res_gelu=False):
+                   out_f32=False, out_sc=1, tag="", res_gelu=False, exact_gelu=False):
         m_tiles = conv_tile_count(NB, H, W)
         kblocks = taps * Cin // 64
         bn = pick_bn(npad, m_tiles, kblocks)
         splits = pick_splits(m_tiles, npad // bn, kblocks, npad)
+        if exact_gelu:
+            # the exact GELU has no stand-alone backward: its dgrad always takes the CONV flags 8 epilogue, which needs one K loop per
+            # tile (no split-K) and tiles of >= 64 columns -- forced here instead of picked (small batches would pick split-K)
+            assert self.exact_gelu_epilogue_ok(npad, Cout), tag
+            bn, splits = max(bn, 64), 1
         cluster = 0
         if splits > 1 and self.cluster_splitk and self.conv_impl in (0, 3) and not out_f32 and out_sc == 1:
             # one launch and no fp32 partial tensor, unless the workspace split would give each CTA a shorter K loop
@@ -333,9 +339,9 @@ class Plan:
             ws = self.new(splits * m_tiles * 128 * npad, "f", "splitk_ws")
         i = [NB, H, W, Cin, Cout, npad, taps, *x_strides, *out_strides, *(res_strides or (0, 0, 0)), bn, splits, self.conv_impl, out_sc,
              0, 0, 0, cluster]  # i20..i22 reserved
-        if res_gelu:
+        if res_gelu and not exact_gelu:
             assert self.conv_gelu_epilogue_ok(NB, H, W, Cin, npad, Cout, taps), tag
-        self.emit("CONV", flags=(1 if out_f32 else 0) | (4 if res_gelu else 0), i=i,
+        self.emit("CONV", flags=(1 if out_f32 else 0) | ((8 if exact_gelu else 4) if res_gelu else 0), i=i,
                   p=[x_ptr, self._bp(wbuf), self._bp(bias), res_ptr, out_ptr, self._bp(ws), None], tag=tag)
 
     def conv_gelu_epilogue_ok(self, NB, H, W, Cin, npad, Cout, taps) -> bool:
@@ -347,6 +353,11 @@ class Plan:
         kblocks = taps * Cin // 64
         bn = pick_bn(npad, m_tiles, kblocks)
         return (m_tiles >= 2 or self.conv_impl == 3) and pick_splits(m_tiles, npad // bn, kblocks, npad) == 1 and bn >= 64 and Cout % 64 == 0
+
+    def exact_gelu_epilogue_ok(self, npad, Cout) -> bool:
+        """can a dgrad take the exact-GELU' epilogue (CONV flags 8)?  Any shape on the wgmma kernels (`_emit_conv` forces BN >= 64 and no
+        split-K for it, and CGD_QGELU_EPI does not apply: there is no other backward); not on the SIMT verification kernel (conv_impl 1)"""
+        return self.conv_impl != 1 and npad % 64 == 0 and Cout % 64 == 0
 
     @staticmethod
     def _strides(a: Act):
@@ -368,14 +379,17 @@ class Plan:
                 self.add_grad(res, dy)
             if w.bwd is None:
                 return
-            u = self._gelu_src.get(x.key())
-            if (u is not None and self.grad_of(x) is None and u.ld == u.C
-                    and self.conv_gelu_epilogue_ok(x.N, x.H, x.W, dy.C, w.bwd_npad, x.C, w.taps)):
-                # x = QuickGELU(u) feeds only this conv: its dgrad epilogue multiplies by QuickGELU'(u) (CONV flags 4) and writes
-                # d u directly -- no d a tensor, no QGELU_BWD launch (quick_gelu's own backward then finds no gradient and emits nothing)
+            u, exact = self._gelu_src.get(x.key(), (None, False))
+            fusable = (self.exact_gelu_epilogue_ok(w.bwd_npad, x.C) if exact
+                       else self.conv_gelu_epilogue_ok(x.N, x.H, x.W, dy.C, w.bwd_npad, x.C, w.taps))
+            if u is not None and self.grad_of(x) is None and u.ld == u.C and fusable:
+                # x = QuickGELU(u) feeds only this conv: its dgrad epilogue multiplies by QuickGELU'(u) (CONV flags 4; GELU'(u), flags 8,
+                # for an exact GELU) and writes d u directly -- no d a tensor, no QGELU_BWD launch (quick_gelu's own backward then finds
+                # no gradient and emits nothing)
                 du = self.act(u.N, u.H, u.W, u.C, "d_" + name + ".gelu")
                 self._emit_conv(self._ap(dy), self._strides(dy), x.N, x.H, x.W, dy.C, w.bwd, w.bwd_npad, x.C, w.taps, None,
-                                self._ap(u), self._strides(u), self._ap(du), self._strides(du), tag="d_" + name + "*gelu'", res_gelu=True)
+                                self._ap(u), self._strides(u), self._ap(du), self._strides(du), tag="d_" + name + "*gelu'", res_gelu=True,
+                                exact_gelu=exact)
                 self.add_grad(u, du)
                 return
             cur, has = self.writable_grad(x)
@@ -553,10 +567,12 @@ class Plan:
         return y
 
     # ------------------------------------------------------------------ attention (head dim 64; 128 / 192 / 256 for the 128^2 checkpoint)
-    def attention(self, qkv: Act, heads: int, T: int, nbatch: int, legacy_order: bool, causal: bool = False, name="attn") -> Act:
+    def attention(self, qkv: Act, heads: int, T: int, nbatch: int, legacy_order: bool, causal: bool = False, name="attn",
+                  scale: Optional[float] = None) -> Act:
         """qkv: [nbatch*T rows, 3C].  legacy_order: per-head [q|k|v] interleave (UNet QKVAttentionLegacy);
         otherwise [q heads | k heads | v heads] (QKVAttention, nn.MultiheadAttention).  causal: query i attends to keys <= i
-        (ATTN_FWD flags 1, the CLIP text tower); forward only."""
+        (ATTN_FWD flags 1, the CLIP text tower); forward only.  scale: the softmax scale, 1 / sqrt(head dim) by default (a tower whose
+        heads are zero-padded to a wider kernel head dim passes its own, vit.py)."""
         C = qkv.C // 3
         d = C // heads
         assert d in (64, 128, 192, 256), f"attention kernels support head dims 64 / 128 / 192 / 256, got {d}"
@@ -567,7 +583,7 @@ class Plan:
         else:
             hs, qo, ko, vo = d, 0, C, 2 * C
         ii = [nbatch, heads, T, d, T * qkv.ld, qkv.ld, hs, T * out.ld, out.ld, d]
-        scale = 1.0 / math.sqrt(d)
+        scale = 1.0 / math.sqrt(d) if scale is None else float(scale)
         q = (qkv.buf, qkv.eoff + qo)
         k = (qkv.buf, qkv.eoff + ko)
         v = (qkv.buf, qkv.eoff + vo)
@@ -660,16 +676,21 @@ class Plan:
         self._tape.append(bwd)
         return y
 
-    def quick_gelu(self, u: Act, name="gelu") -> Act:
+    def quick_gelu(self, u: Act, name="gelu", exact=False) -> Act:
+        """QuickGELU, or with `exact` the erf GELU (QGELU_FWD flags 1).  The backward of either is normally fused into the consuming
+        conv's dgrad epilogue (CONV flags 4 / 8); only QuickGELU has a stand-alone backward op."""
         assert u.ld == u.C
         a = self.act(u.N, u.H, u.W, u.C, name)
-        self.emit("QGELU_FWD", i=[u.rows * u.C], p=[self._ap(u), self._ap(a)], tag=name)
-        self._gelu_src[a.key()] = u
+        self.emit("QGELU_FWD", flags=1 if exact else 0, i=[u.rows * u.C], p=[self._ap(u), self._ap(a)], tag=name)
+        self._gelu_src[a.key()] = (u, exact)
 
         def bwd():
             da = self.grad_of(a)
             if da is None:
                 return
+            if exact:
+                raise NotImplementedError(f"{name}: the exact GELU's backward runs only in the dgrad epilogue (CONV flags 8) of a single "
+                                          "consuming conv on the wgmma kernels; the SIMT verification kernel (conv_impl=1) has none")
             assert da.ld == da.C
             du = self.act(u.N, u.H, u.W, u.C, "d_" + name)
             self.emit("QGELU_BWD", i=[u.rows * u.C], p=[self._ap(da), self._ap(u), self._ap(du)], tag="d_" + name)

@@ -5,7 +5,7 @@ run once per text prompt set and run, outside the sampling loop.  The weights ar
 visual tower loads (upstream key layout: ``token_embedding``, ``positional_embedding``, ``transformer.resblocks.N``, ``ln_final``,
 ``text_projection``).  The ops, in order:
 
-    TOKEN_EMBED -> layers x (ln_1, qkv, causal ATTN_FWD, out_proj + residual, ln_2, c_fc, QuickGELU, c_proj + residual)
+    TOKEN_EMBED -> layers x (ln_1, qkv, causal ATTN_FWD, out_proj + residual, ln_2, c_fc, QuickGELU (GELU: OpenCLIP), c_proj + residual)
     -> ROW_GATHER of each sequence's end-of-text row -> ln_final -> fp32 text_projection (LINEAR_SMALL)
 
 Linear layers run on the wgmma GEMM kernel with fp16 operands and fp32 accumulation, like the ViT (the reference's CUDA path loads
@@ -28,15 +28,17 @@ class TextConfig:
     context_length: int = 77
     vocab_size: int = 49408
     output_dim: int = 512
+    act: str = "quick_gelu"  # the MLP's activation: "quick_gelu" (OpenAI CLIP) or "gelu" (exact erf GELU, OpenCLIP)
 
     @property
     def heads(self):
         return self.width // 64
 
 
-def text_config_from_state_dict(sd: dict) -> TextConfig:
+def text_config_from_state_dict(sd: dict, act: str = "quick_gelu") -> TextConfig:
     """clip.model.build_model's reading of the text half: width = ln_final size, heads = width / 64, layers = the non-visual
-    transformer.resblocks.N, context = positional_embedding rows, vocab = token_embedding rows, D = text_projection columns"""
+    transformer.resblocks.N, context = positional_embedding rows, vocab = token_embedding rows, D = text_projection columns.  The MLP
+    activation is not in the keys: `act` ("gelu" for the OpenCLIP towers)"""
     need = ("token_embedding.weight", "positional_embedding", "ln_final.weight", "text_projection")
     missing = [k for k in need if k not in sd]
     if missing:
@@ -44,7 +46,7 @@ def text_config_from_state_dict(sd: dict) -> TextConfig:
                          "checkpoint, or pass target_embeds= / weights=")
     layers = len({k.split(".")[2] for k in sd if k.startswith("transformer.resblocks.")})
     return TextConfig(width=sd["ln_final.weight"].shape[0], layers=layers, context_length=sd["positional_embedding"].shape[0],
-                      vocab_size=sd["token_embedding.weight"].shape[0], output_dim=sd["text_projection"].shape[1])
+                      vocab_size=sd["token_embedding.weight"].shape[0], output_dim=sd["text_projection"].shape[1], act=act)
 
 
 class TextB200:
@@ -88,7 +90,7 @@ class TextB200:
             x = p.conv(a, self._pack(pre, ".attn.out_proj.weight", ".attn.out_proj.bias"), res=x, name=pre + ".out_proj")
             y = p.layer_norm(x, self._const(pre + ".ln_2.weight"), self._const(pre + ".ln_2.bias"), name=pre + ".ln_2")
             u = p.conv(y, self._pack(pre, ".mlp.c_fc.weight", ".mlp.c_fc.bias"), name=pre + ".c_fc")
-            g = p.quick_gelu(u, name=pre + ".gelu")
+            g = p.quick_gelu(u, name=pre + ".gelu", exact=cfg.act == "gelu")
             x = p.conv(g, self._pack(pre, ".mlp.c_proj.weight", ".mlp.c_proj.bias"), res=x, name=pre + ".c_proj")
         eot = Act(p.new(n * w, "h", "eot"), 0, 1, 1, n, w, w)
         p.emit("ROW_GATHER", i=[n, w, x.ld, eot.ld, rows], p=[(x.buf, x.eoff), (self.eot_rows, 0), (eot.buf, 0)], tag="eot_rows")

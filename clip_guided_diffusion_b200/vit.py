@@ -9,11 +9,17 @@ softmax and the final projection are fp32.
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass
+from typing import NamedTuple
 
 import torch as th
 
 from .plan import Act, Plan, pack_conv, _round_up
+from .text import TextConfig
+
+# head dims the attention kernels take (csrc/attention*.cu); a narrower head is zero-padded to the next one (`ViTConfig.head_pad`)
+_KERNEL_HEAD_DIMS = (64, 128)
 
 
 @dataclass
@@ -23,10 +29,17 @@ class ViTConfig:
     width: int = 768
     layers: int = 12
     output_dim: int = 512
+    head_width: int = 64
+    act: str = "quick_gelu"  # the MLP's activation: "quick_gelu" (OpenAI CLIP) or "gelu" (exact erf GELU, OpenCLIP)
 
     @property
     def heads(self):
-        return self.width // 64
+        return self.width // self.head_width
+
+    @property
+    def head_pad(self):
+        """the head dim the attention kernel runs: head_width, or the next kernel head dim with zero rows / columns (ViT-H's 80 -> 128)"""
+        return next(d for d in _KERNEL_HEAD_DIMS if d >= self.head_width)
 
     @property
     def grid(self):
@@ -48,6 +61,71 @@ VIT_CONFIGS = {
     "ViT-L/14": ViTConfig(224, 14, 1024, 24, 768),
     "ViT-L/14@336px": ViTConfig(336, 14, 1024, 24, 768),  # in CLIP_MODEL_URLS (cgd/clip_util.py:28): 24 x 24 patches + class token = 577 tokens
 }
+
+
+class OpenClipConfig(NamedTuple):
+    vision: ViTConfig
+    text: TextConfig
+
+
+# LAION's OpenCLIP ViT models (open_clip/model_configs/<arch>.json), reached through the tower names "open_clip:<arch>".  Their checkpoints
+# use OpenAI's key layout, but every model without the -quickgelu suffix has exact GELU MLPs, and ViT-H-14 has 16 heads of 80.
+OPEN_CLIP_CONFIGS = {
+    "ViT-B-32": OpenClipConfig(ViTConfig(224, 32, 768, 12, 512, act="gelu"), TextConfig(512, 12, output_dim=512, act="gelu")),
+    "ViT-B-32-quickgelu": OpenClipConfig(ViTConfig(224, 32, 768, 12, 512), TextConfig(512, 12, output_dim=512)),
+    "ViT-B-16": OpenClipConfig(ViTConfig(224, 16, 768, 12, 512, act="gelu"), TextConfig(512, 12, output_dim=512, act="gelu")),
+    "ViT-L-14": OpenClipConfig(ViTConfig(224, 14, 1024, 24, 768, act="gelu"), TextConfig(768, 12, output_dim=768, act="gelu")),
+    "ViT-H-14": OpenClipConfig(ViTConfig(224, 14, 1280, 32, 1024, head_width=80, act="gelu"), TextConfig(1024, 24, output_dim=1024, act="gelu")),
+}
+
+
+def _expect(sd: dict, key: str, shape, what: str):
+    if key not in sd:
+        raise ValueError(f"{what}: the state_dict has no {key!r}")
+    if tuple(sd[key].shape) != tuple(shape):
+        raise ValueError(f"{what}: {key!r} has shape {tuple(sd[key].shape)}, the architecture needs {tuple(shape)}")
+
+
+def _block_shapes(pre: str, w: int) -> dict:
+    return {pre + ".attn.in_proj_weight": (3 * w, w), pre + ".mlp.c_fc.weight": (4 * w, w), pre + ".mlp.c_proj.weight": (w, 4 * w)}
+
+
+def check_open_clip_state_dict(arch: str, sd: dict, text: bool = False):
+    """ValueError naming the first key of `sd` that does not fit OPEN_CLIP_CONFIGS[arch]: conv1, the positional embedding, the layer count,
+    every block's in_proj / c_fc / c_proj, proj, and with `text` the text half (token and positional embeddings, layers, text_projection)"""
+    v, t = OPEN_CLIP_CONFIGS[arch]
+    what = f"open_clip:{arch}"
+    w = v.width
+    _expect(sd, "visual.conv1.weight", (w, 3, v.patch_size, v.patch_size), what)
+    _expect(sd, "visual.positional_embedding", (v.tokens, w), what)
+    layers = len({k.split(".")[3] for k in sd if k.startswith("visual.transformer.resblocks.")})
+    if layers != v.layers:
+        raise ValueError(f"{what}: 'visual.transformer.resblocks.*' has {layers} layers, the architecture {v.layers}")
+    for li in range(v.layers):
+        for k, s in _block_shapes(f"visual.transformer.resblocks.{li}", w).items():
+            _expect(sd, k, s, what)
+    _expect(sd, "visual.proj", (w, v.output_dim), what)
+    if text:
+        tw = t.width
+        _expect(sd, "token_embedding.weight", (t.vocab_size, tw), what)
+        _expect(sd, "positional_embedding", (t.context_length, tw), what)
+        layers = len({k.split(".")[2] for k in sd if k.startswith("transformer.resblocks.")})
+        if layers != t.layers:
+            raise ValueError(f"{what}: 'transformer.resblocks.*' has {layers} layers, the text architecture {t.layers}")
+        for li in range(t.layers):
+            for k, s in _block_shapes(f"transformer.resblocks.{li}", tw).items():
+                _expect(sd, k, s, what)
+        _expect(sd, "text_projection", (tw, t.output_dim), what)
+
+
+def pad_heads(t: th.Tensor, heads: int, hw: int, hp: int, dim: int) -> th.Tensor:
+    """zero-pad every head's `hw` entries along `dim` to `hp`: [.., groups * heads * hw, ..] -> [.., groups * heads * hp, ..] (groups = the
+    q / k / v blocks of in_proj, 1 for out_proj's input columns)"""
+    t = t.movedim(dim, 0)
+    g = t.shape[0] // (heads * hw)
+    out = t.new_zeros((g, heads, hp) + tuple(t.shape[1:]))
+    out[:, :, :hw] = t.reshape((g, heads, hw) + tuple(t.shape[1:]))
+    return out.reshape((g * heads * hp,) + tuple(t.shape[1:])).movedim(0, dim)
 
 
 def vit_config_from_state_dict(sd: dict) -> ViTConfig:
@@ -91,11 +169,21 @@ class ViTB200:
         return self._ccache[key]
 
     def _pack(self, wkey, bkey, name, **kw):
+        """pad="rows": every head's q, k and v rows (and bias entries) zero-padded to the kernel head dim; pad="cols": every head's input
+        columns (out_proj).  Zero k / v columns add nothing to q.k or to the output, and their dgrads are exactly zero."""
         if name not in self._wcache:
             w = self._w(wkey)
+            b = self._w(bkey) if bkey else None
             if kw.pop("flatten", False):
                 w = w.reshape(w.shape[0], -1)
-            self._wcache[name] = pack_conv(self.plan, w, self._w(bkey) if bkey else None, name=name, **kw)
+            pad, cfg = kw.pop("pad", None), self.cfg
+            if pad and cfg.head_pad != cfg.head_width:
+                hp = (cfg.heads, cfg.head_width, cfg.head_pad)
+                if pad == "rows":
+                    w, b = pad_heads(w, *hp, dim=0), pad_heads(b, *hp, dim=0)
+                else:
+                    w = pad_heads(w, *hp, dim=1)
+            self._wcache[name] = pack_conv(self.plan, w, b, name=name, **kw)
         return self._wcache[name]
 
     def part_ranges(self, which: str):
@@ -145,12 +233,13 @@ class ViTB200:
         for li in range(cfg.layers):
             pre = f"transformer.resblocks.{li}"
             y = p.layer_norm(x, self._const(pre + ".ln_1.weight"), self._const(pre + ".ln_1.bias"), name=pre + ".ln_1")
-            qkv = p.conv(y, self._pack(pre + ".attn.in_proj_weight", pre + ".attn.in_proj_bias", pre + ".in_proj"), name=pre + ".qkv")
-            a = p.attention(qkv, cfg.heads, T, n, legacy_order=False, name=pre + ".attn")
-            x = p.conv(a, self._pack(pre + ".attn.out_proj.weight", pre + ".attn.out_proj.bias", pre + ".out_proj"), res=x, name=pre + ".out_proj")
+            qkv = p.conv(y, self._pack(pre + ".attn.in_proj_weight", pre + ".attn.in_proj_bias", pre + ".in_proj", pad="rows"), name=pre + ".qkv")
+            a = p.attention(qkv, cfg.heads, T, n, legacy_order=False, name=pre + ".attn", scale=1.0 / math.sqrt(cfg.head_width))
+            x = p.conv(a, self._pack(pre + ".attn.out_proj.weight", pre + ".attn.out_proj.bias", pre + ".out_proj", pad="cols"), res=x,
+                       name=pre + ".out_proj")
             y = p.layer_norm(x, self._const(pre + ".ln_2.weight"), self._const(pre + ".ln_2.bias"), name=pre + ".ln_2")
             u = p.conv(y, self._pack(pre + ".mlp.c_fc.weight", pre + ".mlp.c_fc.bias", pre + ".c_fc"), name=pre + ".c_fc")
-            g = p.quick_gelu(u, name=pre + ".gelu")
+            g = p.quick_gelu(u, name=pre + ".gelu", exact=cfg.act == "gelu")
             x = p.conv(g, self._pack(pre + ".mlp.c_proj.weight", pre + ".mlp.c_proj.bias", pre + ".c_proj"), res=x, name=pre + ".c_proj")
         # ln_post on the class token of every image, then the fp32 projection
         c = p.layer_norm(x, self._const("ln_post.weight"), self._const("ln_post.bias"), rows=n, ldx=T * w, name="ln_post")

@@ -67,7 +67,8 @@ enum {
    *   i23 = 1: split-K inside a thread-block cluster of `splits` CTAs, reduced through distributed shared memory (one launch, no
    *   workspace; splits in 2..8, BN >= 64, BN / splits a multiple of 16, fp16 contiguous output, Cout % 8 == 0)
    *   flags: 1 = out is fp32 ; 2 reserved (0) ; 4 = p3 is a QuickGELU pre-activation u and out = acc * QuickGELU'(u) instead of acc + res
-   *   (dgrad of the CLIP MLP's c_proj writing d c_fc directly; wgmma kernel, no split-K, Cout % 8 == 0, no bias) */
+   *   (dgrad of the CLIP MLP's c_proj writing d c_fc directly; wgmma kernel, no split-K, Cout % 8 == 0, no bias) ; 8 = the same with the
+   *   exact GELU: out = acc * (Phi(u) + u phi(u)) (the OpenCLIP towers' MLPs; same preconditions; 4 | 8 is rejected) */
   CGD_OP_CONV = 1,
   /* GroupNorm(32) statistics: per (image, chunk, group) partial sum / sum of squares; the last block per image
    * folds the chunks (fixed order, fp64) into (mean, rstd).  [3P] GroupNorm32 (SURVEY K5).
@@ -121,7 +122,8 @@ enum {
   CGD_OP_LN_FWD = 16,
   /* p0 dy p1 x p2 gamma p3 stats p4 dx ; i0 rows i1 w i2 ld_dy i3 ldx i4 ld_dx ; flags 2 = accumulate */
   CGD_OP_LN_BWD = 17,
-  /* QuickGELU a = u*sigmoid(1.702u): p0 u p1 a ; i0 n (contiguous) */
+  /* QuickGELU a = u*sigmoid(1.702u): p0 u p1 a ; i0 n (contiguous) ; flags 1 = exact GELU a = 0.5 u (1 + erf(u / sqrt 2)) instead (fp32
+   * from the fp16 u, one rounding to fp16; the OpenCLIP towers), any other flag bit is rejected */
   CGD_OP_QGELU_FWD = 18,
   /* p0 da p1 u p2 du ; i0 n */
   CGD_OP_QGELU_BWD = 19,

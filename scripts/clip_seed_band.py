@@ -10,7 +10,8 @@ band]).  The arena holds every intermediate gradient of the backward, so for eac
 The chosen band is the largest one that leaves at least 2^4 of headroom in every tower.  Seeded weights are not the published
 checkpoints: the band rests on seeded towers.
 
-    python scripts/clip_seed_band.py      # prints one JSON line, with the card's name and power limit
+    python scripts/clip_seed_band.py                     # prints one JSON line, with the card's name and power limit
+    python scripts/clip_seed_band.py open_clip:ViT-H-14  # other towers: any VIT_CONFIGS / RN_CONFIGS / "open_clip:<arch>" names
 """
 from __future__ import annotations
 
@@ -34,7 +35,10 @@ BANDS = [2.0 ** k for k in range(16)]
 
 
 def measure(name, n=16):
-    if name in pv.VIT_CONFIGS:
+    if name.startswith("open_clip:"):
+        cfg = pv.OPEN_CLIP_CONFIGS[name[len("open_clip:"):]].vision
+        sd = pw.seeded_state_dict(pw.vit_param_shapes(cfg), 1235)
+    elif name in pv.VIT_CONFIGS:
         cfg = pv.VIT_CONFIGS[name]
         sd = pw.seeded_state_dict(pw.vit_param_shapes(cfg), 1235)
     else:
@@ -72,12 +76,15 @@ def main():
     if not th.cuda.is_available():
         raise SystemExit("needs a GPU")
     res = {"card": card(), "images": 16, "weights": "seeded (pw.seeded_state_dict / seeded_rn_state_dict), not the published checkpoints"}
-    res["towers"] = {name: measure(name) for name in TOWERS}
+    res["towers"] = {name: measure(name) for name in (sys.argv[1:] or TOWERS)}
     ok = [b for b in BANDS if all(r["headroom_log2"] is not None and r["headroom_log2"] >= 4
                                   for t in res["towers"].values() for r in t["bands"] if r["band"] == b)]
     res["chosen_band"] = max(ok) if ok else None
     if ok:
         res["headroom_log2_at_chosen"] = min(r["headroom_log2"] for t in res["towers"].values() for r in t["bands"] if r["band"] == max(ok))
+    # every tower's headroom at the band the package ships
+    res["headroom_log2_at_shipped_band"] = {name: next(r["headroom_log2"] for r in t["bands"] if r["band"] == cm.CLIP_SEED_BAND)
+                                           for name, t in res["towers"].items()}
     print(json.dumps(res))
 
 
